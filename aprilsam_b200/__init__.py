@@ -1,4 +1,4 @@
-"""aprilsam_b200: B200-native replacement for AprilSAM's april_graph_cholesky{,_inc} path.
+"""aprilsam_b200: H100-native (sm_90a) replacement for AprilSAM's april_graph_cholesky{,_inc} path.
 
 The product is the C/CUDA shared library `libaprilsam_b200.so` (drop-in for the reference's
 libaprilsam public API, see include/aprilsam/aprilsam.h and INTEGRATION.md).  This Python

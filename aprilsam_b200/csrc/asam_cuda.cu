@@ -1,4 +1,4 @@
-// asam_cuda.cu -- C-ABI (include/asam_cuda.h) of the sm_100a CUDA implementation of the AprilSAM
+// asam_cuda.cu -- C-ABI (include/asam_cuda.h) of the sm_90a CUDA implementation of the AprilSAM
 // Gauss-Newton path: device context, HBM buffers, uploads/downloads, kernel launches.
 // The kernels themselves are in asam_kernels.cuh.
 //
@@ -130,7 +130,7 @@ struct asam_dev {
 
     // launch config
     int fac_threads = 256, fac_grid = 0, fac_smem = 0;
-    int bs_threads = 256, bs_grid = 0, bs_smem = 0; // 8 warps: measured 0.153 -> 0.131 ms (M3500), 1.95 -> 1.37 ms (100 k) vs 4 warps; ASAM_BS_THREADS=128 for comparison
+    int bs_threads = 256, bs_grid = 0, bs_smem = 0; // 8 warps: faster than 4 on M3500 and the 100 k world in A/B runs; ASAM_BS_THREADS=128 for comparison
 
     int64_t n_launch = 0, n_h2d = 0, n_d2h = 0;
 
@@ -1482,11 +1482,11 @@ ASAM_EXPORT int asam_timer_stop(asam_dev_t *d, float *ms)
     return 0;
 }
 
-// Evict the working set from L2 between timed iterations: overwrite a buffer larger than L2.
+// Evict the working set from L2 between timed iterations: overwrite a buffer larger than L2 (H100: 50 MB).
 ASAM_EXPORT int asam_l2_flush(asam_dev_t *d)
 {
     CK(cudaSetDevice(d->device));
-    const size_t bytes = (size_t) 384 << 20;
+    const size_t bytes = (size_t) 128 << 20;
     if (buf_reserve(d, d->flush, bytes, false, false) || flush_uploads(d))
         return 1;
     d->flush_val ^= 0x5a;

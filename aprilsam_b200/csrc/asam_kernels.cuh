@@ -1,4 +1,4 @@
-// asam_kernels.cuh -- device code of the AprilSAM Gauss-Newton path for sm_100a.
+// asam_kernels.cuh -- device code of the AprilSAM Gauss-Newton path for sm_90a (H100).
 //
 //   k_linearize   one thread per factor: residual, Jacobians, J'WJ / J'Wr, atomically
 //                 scattered into the block Hessian (Adiag / Aoff / Bq).
@@ -330,7 +330,7 @@ struct FacArgs {
     unsigned long long *trace; // optional: 8 words per task
     int pb_smem;   // panel width of shared-memory fronts (multiple of 3)
     int smem_mma;  // shared-memory fronts on the FP64 tensor pipe: 1 = the one wide update of kept columns (incremental
-                   // steps: k_step's factor phase 17.6 -> 15.0 us), 2 = also the 12-column panel updates, 0 = DFMA only
+                   // steps), 2 = also the 12-column panel updates, 0 = DFMA only
     int staged;    // tile mode 3: publish L11 in 12-column stages (0: all at once)
     int tile_mode; // trailing-update tiles of the team path: 0 DFMA, 1 mma.sync f64, 2 mma.sync f64 + bulk async copies
     int solo_pb; // widest staged panel of a front that one CTA handles out of HBM (multiple of ASAM_PB)
@@ -461,7 +461,7 @@ __device__ __forceinline__ void trailing_update_mma(double *C, const int ld, con
 __device__ __forceinline__ void bar_sub(const int nthreads) { asm volatile("bar.sync 1, %0;" ::"r"(nthreads) : "memory"); }
 
 // (tuning switches live in CONSTANT memory: a __device__ global read inside panel_factor is a global load on the
-// dependent chain of every 3x3 step -- measured +2.3 us per 48 x 48 diagonal block)
+// dependent chain of every 3x3 step)
 __constant__ int g_pf_groups = 1; // ASAM_PF_GROUPS=0: one thread per row in the in-panel update of panel_factor (A/B)
 __constant__ int g_dmap_ahead = 1; // ASAM_DMAP_AHEAD=0: destination maps child by child inside the extend-add loop (A/B)
 __constant__ int g_diag_mma = 1;  // ASAM_DIAG_MMA=0: DFMA update inside the 48 x 48 diagonal block of the team path (A/B)
@@ -741,7 +741,7 @@ __device__ __noinline__ void tile_mma(double *F, const int ld, const int m, cons
 // buffers of (m+2) rows x ASAM_LDW doubles; buffer k&1 holds the factored panel k by ROWS: row r of the front
 // at W[r * ASAM_LDW .. + pb), zero up to the next multiple of 4.  A tile's operands -- a chunk of rows of the
 // panel -- are then ONE contiguous block each: two bulk asynchronous copies per tile instead of one per panel
-// column (measured: 96 small copies cost ~5 us, as much as staging by hand).  ASAM_LDW = 4 (mod 16) keeps the
+// column (96 small copies cost as much as staging by hand).  ASAM_LDW = 4 (mod 16) keeps the
 // m8n8k4 fragment loads conflict free, and a row is 416 bytes: every row 16-byte aligned.
 #define ASAM_LDW 52
 #define ASAM_WS_DOUBLES(m) (2 * (size_t) ((m) + 2) * ASAM_LDW)
@@ -1310,8 +1310,8 @@ __device__ bool team_front(const FacArgs &a, const asam_sn_desc_t &d, int s, int
             // and go to the front + the flag (8 * seq + stage); the crew solves the matching 12 columns of its rows
             // while the next sub-panel is being factored, instead of starting when all 48 are done
             constexpr int LDD = ASAM_TPB;
-            constexpr int SUB = 256; // threads that factor the block (measured: 64 threads on a two-warp barrier are SLOWER,
-                                     // 20.3 vs 15.7 us per block: the publish / update loops want the threads more than the barriers cost)
+            constexpr int SUB = 256; // threads that factor the block (64 threads on a two-warp barrier were SLOWER:
+                                     // the publish / update loops want the threads more than the barriers cost)
             int stage = 0;
             if (tid < SUB) {
                 for (int k1 = 0; k1 < pb; k1 += ASAM_PB) {
@@ -1370,9 +1370,9 @@ __device__ bool team_front(const FacArgs &a, const asam_sn_desc_t &d, int s, int
             // Two groups of four warps.  LOADERS (warps 4-7): wait for the flag of stage s, fetch its 12 columns of L11
             // (one L2 round trip) into D and hand them over on named barrier 3 + s (they only arrive).  SOLVERS (warps
             // 0-3, one row each): pick the columns up and solve.  The loaders are already polling for stage s + 1 while
-            // the solvers work on s: a stage costs the crew max(poll + fetch, solve) instead of their sum -- measured
-            // before: 5 us per stage against a block published every 3.9 us, the row chunks finished 9 us after the
-            // last publish and the whole team waited for them.
+            // the solvers work on s: a stage costs the crew max(poll + fetch, solve) instead of their sum -- before,
+            // a stage took longer than the block took to publish it, the row chunks finished well after the last
+            // publish and the whole team waited for them.
             if (tid == 0)
                 *s_flag = 1;
             __syncthreads();
@@ -1857,7 +1857,7 @@ __device__ bool cta_front(const FacArgs &a, const int t, const int s, const int 
                 accA += tb - ta;
             }
             const int n = m - (k0 + pb);
-            if (a.smem_mma >= 2 && n > 0) // (measured: 12-column panels are faster on the DFMA tiles -- M3500 0.435 vs 0.459 ms)
+            if (a.smem_mma >= 2 && n > 0) // (12-column panels were faster on the DFMA tiles in A/B runs)
                 trailing_update_mma(F, ld, P, ld, pb, k0 + pb, m, m);
             else if (n > 48)
                 trailing_update<2, 8>(F, ld, P, ld, pb, k0 + pb, m, m);

@@ -117,7 +117,7 @@ typedef struct {
      * (+ the top in btasks); see build_schedule() in plan.c */
     int world, rank;
     int max_team;   /* largest CTA team k_factor can seat (resident CTAs of the device; 0 = default) */
-    int n_cta;      /* resident CTAs of k_factor on the device (0 = 148): processors of the simulated schedule */
+    int n_cta;      /* resident CTAs of k_factor on the device (0 = 132, the SMs of an H100): processors of the simulated schedule */
     int *top_tasks, *top_nwait;
     int n_top, n_top_sn;
     int n_shards;

@@ -53,7 +53,7 @@ ASAM_API void matd_destroy(matd_t *m) { free(m); }
 ASAM_API void APRILSAM_VERSION(void)
 {
     printf("=========================\n");
-    printf("| APRILSAM-B200 (sm_100a) |\n");
+    printf("| APRILSAM-B200 (sm_90a)  |\n");
     printf("=========================\n\n");
 }
 

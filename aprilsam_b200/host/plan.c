@@ -48,7 +48,7 @@ void asam_dbg_build_profile(double *out, int reset)
 #define RELAX_FILL 24 /* ... and explicit zero blocks (3x3) added per merge */
 #define TEAM_MERGE_PCT 20     /* team-sized fronts: extra rows tolerated per merge, % of the front (0: off; swept 10 .. 60) */
 #define TEAM_MERGE_MFLOP 400.0 /* ... and extra flops per merge (millions) */
-#define ASAM_TEAM_ROOM 100       /* CTAs that the team fronts of one tree level may claim together (swept: 100 / 120 / 148 / 220) */
+#define ASAM_TEAM_ROOM 80        /* CTAs that the team fronts of one tree level may claim together (H100, 100 k dense world: 80 beats 100 and 132) */
 #define ASAM_BSLEAF_MAX 64       /* = ASAM_BSL_XS of k_backsolve_leaf: own columns / rows below */
 #define ASAM_BSLEAF_MIN_COUNT 4096 /* measured: no gain on M3500-sized trees (the kernel boundary eats it) */
 #define ASAM_LEAF_MAX_M_DEFAULT 63 /* <= ASAM_LEAF_M of k_factor_leaf (ASAM_LEAF_MAX_M overrides downwards, tuning) */
@@ -268,8 +268,8 @@ static void fslot_reserve(plan_t *pl, int n)
 
 /* rel[k] for k >= cb: index of the child's row in the parent's row list */
 /* Largest front of the warp-per-front kernel.  Big trees are bound by CTA-time (every front the leaf kernel takes frees an
- * SM for 10-15 us: 100 k dense world 5.64 -> 5.49 ms with 63 instead of 48), small ones by their dependent chain, where
- * a longer leaf launch ahead of k_factor only adds to it (30 k world 2.99 -> 3.07 ms): the wider limit from
+ * SM for a team front), small ones by their dependent chain, where
+ * a longer leaf launch ahead of k_factor only adds to it: the wider limit from
  * ASAM_LEAF_WIDE_MIN_SN supernodes on.  ASAM_LEAF_MAX_M overrides (tuning). */
 #define ASAM_LEAF_WIDE_MIN_SN 30000
 static int leaf_max_m_for(int nsn)
@@ -303,7 +303,7 @@ int asam_host_threads(void)
         int want = e && atoi(e) > 0 ? atoi(e) : PLAN_OMP_THREADS;
         want = want > 16 ? 16 : want;
         if (want > 1) {
-            /* two threads spinning for ~0.1 ms each: side by side that takes as long as one of them */
+            /* two threads spinning for a fixed count each: side by side that takes as long as one of them */
             const int iters = 40000;
             double t0 = host_now_ms();
             host_spin(iters);
@@ -383,7 +383,7 @@ static void emit_segment(plan_t *pl, int s, ivec_t *buf, int64_t base)
  * Larger ones are bound by the LATENCY of their panel steps (two team barriers, the diagonal
  * block, one trailing tile per worker), not by throughput: the team gets one CTA per 256 x 64
  * tile of the first trailing update and no more, so that the fronts of one tree level find room
- * side by side on the 148 SMs instead of queueing for each other's workers. */
+ * side by side on the SMs instead of queueing for each other's workers. */
 static int front_fits_smem(int mb)
 {
     int64_t m = 3 * (int64_t) mb;
@@ -392,9 +392,8 @@ static int front_fits_smem(int mb)
 
 /* Fronts up to this order that do not fit in shared memory are still handled by ONE CTA (out of
  * HBM/L2, wide staged panels: cta_front's second mode): a team pays two barriers and several L2 round
- * trips per 48 columns, which for a few hundred rows is all latency -- measured 96 us x 2.2 CTAs per
- * front of order 160-300 in the 100 k world, where 740 such fronts queue for the SMs.  ASAM_SOLO_MAX_M
- * overrides (tuning). */
+ * trips per 48 columns, which for a few hundred rows is all latency -- in the 100 k world 740 fronts of
+ * order 160-300 queue for the SMs.  ASAM_SOLO_MAX_M overrides (tuning). */
 static int solo_max_m(void)
 {
     static int v = -1;
@@ -414,8 +413,8 @@ static int team_size(int mb, int cb, int cap)
     for (int64_t cb0 = j0; cb0 < m; cb0 += 64)
         tiles += (m - cb0 + 1 + 255) / 256;
     int64_t chunks = 1 + (m - j0 + 1 + 127) / 128; /* look-ahead crew: the diagonal block + the 128-row chunks (ASAM_CROWS) */
-    /* A panel step lasts ~30 us (diagonal block + row solves + barrier: the dependent chain), a tensor-pipe tile
-     * ~4-5 us: a worker outside the crew gets through several tiles per step, and a worker that has none left only
+    /* A panel step (diagonal block + row solves + barrier: the dependent chain) lasts several times as long as a
+     * tensor-pipe tile: a worker outside the crew gets through several tiles per step, and a worker that has none left only
      * holds an SM that another front could use.  ASAM_TILES_PER_WORKER overrides (tuning). */
     static int tpw = 0;
     if (tpw == 0) {
@@ -540,8 +539,8 @@ static double front_lat_us(const plan_t *pl, int s, int g)
 
 /* ---- static list schedule --------------------------------------------------------------------------
  * The ticket order of k_factor decides when a front's CTAs are taken: a team whose tickets come up while
- * its children are still running spins on all its CTAs (measured on the 100 k world: the nine fronts of
- * order > 1000 held ~50 CTAs each for 218 us before they could start -- an eighth of the kernel's SM time).
+ * its children are still running spins on all its CTAs (on the 100 k world the nine fronts of order > 1000
+ * each hold dozens of CTAs).
  * So the order is taken from a SIMULATION of the kernel: P resident CTAs, every front with its modelled
  * duration and team size, ready fronts started by priority (length of the dependent chain above them) as
  * CTAs become free; the order in which the simulation STARTS the fronts is the ticket order.  Children finish
@@ -778,17 +777,16 @@ static void build_schedule(plan_t *pl)
 
     /* Task order.  The persistent kernels hand out tasks in list order, so the list IS the schedule.  Plain
      * level order (every front of level l before any of level l+1) starts the deepest chain of the tree last
-     * among its level-mates and leaves its top to run alone at the end (measured on the 100 k world: all SMs
-     * busy until 3.3 ms, then a 3.3 ms tail with most of them spinning; on M3500 the critical chain's
-     * level-2 front got its CTA at 50 us of 457).  Critical-path-first instead: fronts are listed by
+     * among its level-mates and leaves its top to run alone at the end, with most SMs spinning.
+     * Critical-path-first instead: fronts are listed by
      * DESCENDING length of the dependent chain from them up to the root (their own modelled latency
      * included), which is still a topological order -- a child's chain is its parent's plus its own -- so a
      * waiting CTA only ever waits for tasks that were handed out before its own.  ASAM_TASK_ORDER=level keeps
      * the level order (A/B). */
     int *byl = malloc(sizeof(int) * (size_t) (nsn + 1));
     int order_mode = 0; /* 0 level, 1 chain length ("cp"), 2 simulated schedule ("sim"), 3 auto: cp or sim by load */
-    int *bylv = malloc(sizeof(int) * (size_t) (nsn + 1)); /* plain level order: the back-substitution list (measured:
-                                                            * 1.15 ms against 1.42 ms with the reversed chain order) */
+    int *bylv = malloc(sizeof(int) * (size_t) (nsn + 1)); /* plain level order: the back-substitution list (faster
+                                                            * than the reversed chain order in A/B runs) */
     {
         int *cnt = calloc((size_t) pl->n_levels + 2, sizeof(int));
         for (int s = 0; s < nsn; s++)
@@ -809,7 +807,7 @@ static void build_schedule(plan_t *pl)
     }
 
     /* team sizes.  A front's team is bound by latency, not throughput (team_size()), so where one tree
-     * level holds more team fronts than the 148 SMs can seat side by side, smaller teams finish the
+     * level holds more team fronts than the SMs can seat side by side, smaller teams finish the
      * LEVEL sooner: CTA-time per front (G x duration) falls with G.  Scale the teams of such a level
      * down to the room there is (never below 2). */
     int *G_of = malloc(sizeof(int) * (size_t) (nsn + 1));
@@ -859,7 +857,7 @@ static void build_schedule(plan_t *pl)
             if (up_us[s] > chain)
                 chain = up_us[s];
         }
-        const int P = pl->n_cta > 0 ? pl->n_cta : 148;
+        const int P = pl->n_cta > 0 ? pl->n_cta : 132;
         /* auto: where the SMs are far from saturated (M3500: 11 of 67 CTA-ms busy) spinning costs nothing and the
          * eager chain-length order starts parents soonest; where they are saturated, a team must not take its
          * CTAs before it can use them */
@@ -958,7 +956,7 @@ static void build_schedule(plan_t *pl)
      * Order inside a segment: by the modelled TIME of the longest chain below a supernode (its own solve included),
      * longest first -- a parent's chain is longer than any child's, so the order is topological, and the deep
      * chains do not queue behind the thousands of supernodes that merely share their height (level order: the
-     * bottom of the longest chain of the 100 k world got its tickets 20 us late per link).  ASAM_BS_ORDER=level
+     * bottom of the longest chain of the 100 k world got its tickets late at every link).  ASAM_BS_ORDER=level
      * keeps the height order (A/B). */
     {
         const char *eb = getenv("ASAM_BS_ORDER");
@@ -1289,7 +1287,7 @@ static int plan_build_impl(plan_t *pl, asam_dev_t *dev, int N, int n_factors, co
             if (!merge && parent[pp] == p && z == 0 && !front_fits_smem(gcb + nbp))
                 merge = 1;
             /* team-sized fronts along a chain: every front boundary costs the chain an extend-add pass, a
-             * first panel without look-ahead, a ticket and a partly filled last panel (~80 us together), the
+             * first panel without look-ahead, a ticket and a partly filled last panel, the
              * explicit zeros of a merge only tensor-pipe tiles spread over the whole team.  Merge while the
              * extra rows stay below team_merge_pct % of the front and the extra flops below team_merge_mflop. */
             if (!merge && parent[pp] == p && team_merge_pct > 0 && !front_fits_smem(gcb + nbp) &&

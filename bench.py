@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- Gauss-Newton solves/sec of the april_graph_cholesky{,_inc} path on B200.
+"""bench.py -- Gauss-Newton solves/sec of the april_graph_cholesky{,_inc} path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
                     [--workload all|manhattan_batch|m3500_batch|m3500_replay|manhattan_replay]
-                    [--poses P] [--replay-from S] [--shard auto|on|off]
+                    [--poses P] [--replay-from S] [--shard auto|on|off] [--dump-outputs DIR]
 
 One "step" is one pass of the hot path over one batch of synthetic/fixture input:
   *_batch   one april_graph_cholesky() call on the full graph (relinearise -> assemble ->
@@ -16,7 +16,10 @@ The metric (BASELINE.json) names four workloads.  The default run (--workload al
 them in ONE JSON line: the headline keys describe `manhattan_batch` (100 k poses / 400 k factors, the
 largest single-GPU configuration; K timed steps exactly), and `workloads` carries one record each for
 `m3500_batch`, `m3500_replay` and `manhattan_replay` (window from pose --replay-from), every one with
-its own value / e2e / roofline / cpu_baseline, timed for >= 1 s.  --workload X measures X alone.
+its own value / e2e / roofline / cpu_baseline.  --steps K times K steps after --warmup W untimed ones in
+EVERY workload (replays: at most the poses left in the graph); without --steps the headline times 20 and
+the others keep windows of their own (M3500 batch 1500 calls, the whole M3500 replay, 1000 replay steps
+of the synthetic world).  --workload X measures X alone.
 
 JSON line (rank 0):
   value        solves/s with every input already resident in HBM: the GPU pipeline
@@ -31,6 +34,10 @@ JSON line (rank 0):
                inside the e2e calls, and the fraction of MEASURED_PEAKS.json hbm_gbs (k_factor also against
                the FP64 peak measured live by asam_measure_fp64_peak)
   cpu_baseline the reference's own CPU implementation (oracle/_ref) on this box, 1 thread
+--dump-outputs DIR (rank 0) writes, after the timed steps, what each workload's timed path computed in its last
+step as DIR/<name>.npy (float64): <workload>_states, the node states a caller of the public API holds after the
+last timed call, and for batch workloads <workload>_x, the solution of the last device-resident step (elimination
+order).  Inputs are seeded fixtures, so two builds run with the same arguments can be compared output for output.
 Multi-GPU (one process per GPU, torchrun).  manhattan_batch shards ONE solve over the GPUs
 (elimination-tree shards per rank, NCCL broadcast of the shard roots' update matrices and of the solution
 segments, the top of the tree replicated -- DESIGN.md section 6): every rank calls april_graph_cholesky
@@ -58,7 +65,7 @@ from aprilsam_b200 import harness as H  # noqa: E402
 
 METRIC = "Gauss-Newton solves/sec (batch + incremental) on M3500 & 100k-pose graph"
 ALL = ["manhattan_batch", "m3500_batch", "m3500_replay", "manhattan_replay"]
-MIN_TIMED_S = 1.0  # sub-workloads: timed region at least this long
+DEFAULT_STEPS = 20  # headline workload without --steps
 
 
 def load_workload(name: str, poses: int):
@@ -85,7 +92,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM HBM3 3.35 TB/s; not reached)"
 
 
 class ClockSampler:
@@ -286,13 +293,13 @@ def run_reference(args, names, world, rank):
     if rank != 0:
         return
     if not H.available("reference"):
-        print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref not built (needs /root/reference at build time)"}))
+        print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref not built (needs the reference sources at build time)"}))
         return
     recs = {}
     for i, name in enumerate(names):
         d, label = load_workload(name, args.poses)
-        if i == 0:
-            steps, warm = args.steps, args.warmup
+        if args.steps is not None or i == 0:
+            steps, warm = DEFAULT_STEPS if args.steps is None else args.steps, args.warmup
         elif name == "m3500_batch":
             steps, warm = 100, 2
         elif name == "m3500_replay":
@@ -357,7 +364,9 @@ def roofline_entries(ctx: Ctx, name: str, pinfo: dict, kern_ms) -> list:
         if k == "k_factor":
             e.update({"flops_per_launch": pinfo["flops"], "fp64_tflops": pinfo["flops"] / t / 1e12,
                       "fp64_peak_tflops": ctx.fp64_peak_tf,
-                      "fp64_peak_source": "measured live (asam_measure_fp64_peak: DFMA loop, 512 thr/SM); tcgen05 has no FP64 kind",
+                      "fp64_peak_source": "measured live (asam_measure_fp64_peak: DFMA loop, 512 thr/SM); fp64_frac is relative "
+                                          "to DFMA -- the trailing updates run on the FP64 tensor pipe, whose H100 peak is about "
+                                          "twice that",
                       "fp64_frac": (pinfo["flops"] / t / 1e12 / ctx.fp64_peak_tf) if ctx.fp64_peak_tf else None,
                       "note": "latency-bound: the dependent chain of supernode levels / panel steps sets the time (DESIGN.md section 4)"})
         out.append(e)
@@ -399,6 +408,7 @@ def bench_batch(ctx: Ctx, name: str, d, label: str, K: int, W: int, sharded: boo
             e2e_ms.append(t)
             kern.append(capi.kernel_ms(dev))
     launches1, h2d1, d2h1 = capi.counters(dev)
+    e2e_last_states = h.states()
     e2e_val = aggregate_rate(dist, local, jobs, len(e2e_ms), float(np.sum(e2e_ms)) / 1e3)
     kern = np.array(kern)
 
@@ -440,6 +450,8 @@ def bench_batch(ctx: Ctx, name: str, d, label: str, K: int, W: int, sharded: boo
         if i >= W:
             dev_ms.append(ms.value)
     launches_dev = capi.counters(dev)[0] - launches_a
+    x_last = np.zeros((N, 3), dtype=np.float64)
+    capi.check(L.asam_download_x(dev, 0, N, x_last.ctypes.data_as(C.POINTER(C.c_double))), "download_x")
     st = C.c_int()
     L.asam_factor_status(dev, C.byref(st))
     if st.value != 0:
@@ -462,7 +474,7 @@ def bench_batch(ctx: Ctx, name: str, d, label: str, K: int, W: int, sharded: boo
            "roofline_kernels": roofline_entries(ctx, name, pinfo, kern),
            "plan": {k: pinfo[k] for k in ("N", "nsn", "n_slots", "n_levels", "max_m", "nnz_l_blocks")},
            "cold_first_call_ms": cold_ms,
-           "cache": "L2 flushed (384 MiB overwrite) between timed device-resident steps"}
+           "cache": "L2 flushed (128 MiB overwrite) between timed device-resident steps"}
     # ---- cpu baseline + parity against it (rank 0, N = 1) ----------------------------------------
     if with_cpu and rank == 0 and world == 1 and H.available("reference"):
         probe, ref_first = time_reference_batch(d, 1, 0, keep_states=True)
@@ -474,6 +486,7 @@ def bench_batch(ctx: Ctx, name: str, d, label: str, K: int, W: int, sharded: boo
         rec["parity"] = {"vs_reference_first_iteration_max_rel": float(np.abs(first_states - ref_first).max() / scale),
                          "tolerance": 1e-6}
     rec["_first_states"] = first_states
+    rec["_outputs"] = {"states": e2e_last_states, "x": x_last}
     return rec
 
 
@@ -532,7 +545,7 @@ def bench_replay(ctx: Ctx, name: str, d, label: str, K: int, W: int, with_cpu: b
                                              "sample": "same steps, the reference AS SHIPPED (wall-clock escalation heuristic "
                                                        "aprilsam.c:556-559 active; non-deterministic, speed reference only)"}
     rec["_chi2_end"] = chi2_end
-    rec["_end_states"] = end_states
+    rec["_outputs"] = {"states": end_states}
     return rec
 
 
@@ -554,10 +567,11 @@ def run_b200(args, names, world, rank, local, dist):
             capi.comm_init_torch(dist, local)
             capi.check(L.asam_comm_set_sharding(1), "asam_comm_set_sharding")
         if i == 0:
-            K, W = args.steps, args.warmup
             sharded_head = sharded
+        if args.steps is not None or i == 0:
+            K, W = DEFAULT_STEPS if args.steps is None else args.steps, args.warmup
         elif name == "m3500_batch":
-            K, W = max(args.steps, 1500), max(args.warmup, 5)
+            K, W = 1500, max(args.warmup, 5)
         elif name == "m3500_replay":
             K, W = d.n_nodes, 0
         else:
@@ -582,6 +596,11 @@ def run_b200(args, names, world, rank, local, dist):
     clocks = sampler.stop() if rank == 0 else {}
     if rank != 0:
         return
+    if args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, r in recs.items():
+            for k, v in r["_outputs"].items():
+                np.save(os.path.join(args.dump_outputs, f"{name}_{k}.npy"), np.asarray(v, dtype=np.float64))
     for r in recs.values():
         for k in [k for k in r if k.startswith("_")]:
             del r[k]
@@ -614,13 +633,16 @@ def main():
     os.environ.setdefault("NCCL_DEBUG", "WARN")  # (NCCL's version banner would otherwise share stdout with the JSON line)
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=None,
+                    help=f"timed steps of every workload (default: {DEFAULT_STEPS} for the headline, own windows for the others)")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default="all", choices=["all"] + ALL)
     ap.add_argument("--poses", type=int, default=100000)
     ap.add_argument("--replay-from", type=int, default=50000, help="manhattan_replay: first timed step")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path computed in its last step as DIR/<name>.npy (rank 0)")
     ap.add_argument("--shard", choices=["auto", "on", "off"], default="auto",
                     help="--gpus N > 1: shard the elimination tree of ONE solve over the GPUs (NCCL) instead of "
                          "running N replicas; auto = on for manhattan_batch (SURVEY.md section 8e)")
@@ -631,8 +653,6 @@ def main():
         rank = int(os.environ.get("RANK", "0"))
         run_reference(args, names, world, rank)
         return
-    if args.warmup < 3:
-        args.warmup = 3
     world, rank, local, dist = dist_setup(args.gpus)
     try:
         run_b200(args, names, world, rank, local, dist)

@@ -8,7 +8,7 @@
  *
  * What runs where: every entry point below is host C; all arithmetic of
  * april_graph_cholesky{,_inc}() and april_graph_chi2() -- linearisation, J'WJ assembly,
- * sparse Cholesky, triangular solves -- runs in sm_100a CUDA kernels behind the C-ABI in
+ * sparse Cholesky, triangular solves -- runs in sm_90a CUDA kernels behind the C-ABI in
  * include/asam_cuda.h.  There is no CPU fallback: without a CUDA device the solver entry
  * points abort with a message.
  */

@@ -1,4 +1,4 @@
-/* asam_cuda.h -- C-ABI between the host solver (C) and the sm_100a CUDA kernels.
+/* asam_cuda.h -- C-ABI between the host solver (C) and the sm_90a CUDA kernels.
  *
  * Plain pointers and sizes only.  Every entry point returns 0 on success, non-zero on
  * failure (text via asam_last_error()).  All calls on one asam_dev_t must come from one

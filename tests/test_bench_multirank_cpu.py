@@ -76,7 +76,8 @@ def test_reference_arm_json_contract():
 def test_reference_arm_default_line_covers_all_four_workloads():
     """The default line (--workload all) headlines the batch solve of the synthetic Manhattan world and carries one
     record each for m3500_batch, m3500_replay (with the as-shipped wall-clock variant beside it) and manhattan_replay,
-    every record with value / e2e / cpu_baseline; replay records with per-naffected-bucket latencies.  Small world here."""
+    every record with value / e2e / cpu_baseline; replay records with per-naffected-bucket latencies.  Small world here;
+without --steps the sub-workloads keep their own windows (the whole M3500 replay)."""
     import json
     import subprocess
     sys.path.insert(0, ROOT)
@@ -84,12 +85,12 @@ def test_reference_arm_default_line_covers_all_four_workloads():
     if not H.available("reference"):
         pytest.skip("reference oracle not built")
     r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--poses", "3000",
-                        "--replay-from", "1500", "--steps", "2", "--warmup", "1"], capture_output=True, text=True, timeout=600)
+                        "--replay-from", "1500", "--warmup", "1"], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stderr[-1000:]
     lines = [l for l in r.stdout.splitlines() if l.startswith("{")]
     assert len(lines) == 1
     j = json.loads(lines[0])
-    assert j["config"]["workload"] == "manhattan_batch" and j["steps"] == 2 and j["impl"] == "reference"
+    assert j["config"]["workload"] == "manhattan_batch" and j["steps"] == 20 and j["impl"] == "reference"
     assert set(j["workloads"]) == {"m3500_batch", "m3500_replay", "manhattan_replay"}
     for name, rec in j["workloads"].items():
         for k in ("value", "unit", "steps", "ms_per_step", "e2e", "cpu_baseline"):

@@ -1,5 +1,8 @@
 """CPU-only tests (-m "not gpu"): ABI surface, host symbolic layer, oracle vs golden vectors.
 
+What the unmodified reference computes is stored in tests/golden/reference_runs.npz: each `ref_*`
+driver below is run on the reference by tools/make_golden.py, and the tests compare with its output.
+
 The numeric checks replay the plan that would be uploaded to HBM with tests/support/emul.py (a
 numpy emulation of the kernels' index arithmetic) -- that validates ordering, elimination tree,
 supernode row lists, relative indices, gather lists and task order without a device.
@@ -118,29 +121,46 @@ def test_m3500_ordering_and_tree_match_golden(m3500):
     assert info["nsn"] <= info["N"] and info["n_slots"] == 5453
 
 
-@pytest.mark.parametrize("n", [1, 2, 3, 4, 7, 13, 64, 257, 900])
+def reference(key):
+    return golden("reference_runs.npz")[key]
+
+
+def load_m3500():
+    return H.PoseGraphData.load(os.path.join(ROOT, "tests", "golden", "m3500.npz"))
+
+
+SUBGRAPH_SIZES = [1, 2, 3, 4, 7, 13, 64, 257, 900]
+
+
+def ref_subgraph_ordering(impl):
+    out = {}
+    for n in SUBGRAPH_SIZES:
+        with H.Harness(impl) as h:
+            h.load_full(load_m3500().head(n))
+            h.batch()
+            out[f"n{n}_ordering"], out[f"n{n}_parents"] = h.ordering(), h.tree_parents()
+    return out
+
+
+@pytest.mark.parametrize("n", SUBGRAPH_SIZES)
 def test_subgraph_ordering_matches_reference(m3500, n):
-    if not H.available("reference"):
-        pytest.skip("reference oracle not built")
     sub = m3500.head(n)
-    with H.Harness("reference") as h:
-        h.load_full(sub)
-        h.batch()
-        ref_order, ref_par = h.ordering(), h.tree_parents()
     ftype, fa, fb, _, _ = factor_arrays(sub)
     p = HostPlan().build(n, ftype, fa, fb)
-    assert np.array_equal(p.array("order"), ref_order)
-    assert np.array_equal(node_parents(p, n), ref_par)
+    assert np.array_equal(p.array("order"), reference(f"subgraph_ordering__n{n}_ordering"))
+    assert np.array_equal(node_parents(p, n), reference(f"subgraph_ordering__n{n}_parents"))
+
+
+def ref_synthetic_ordering(impl):
+    with H.Harness(impl) as h:
+        h.load_full(datasets.manhattan_dense(1500, seed=3))
+        h.batch()
+        return {"ordering": h.ordering()}
 
 
 def test_synthetic_ordering_matches_reference():
-    if not H.available("reference"):
-        pytest.skip("reference oracle not built")
+    ref_order = reference("synthetic_ordering__ordering")
     d = datasets.manhattan_dense(1500, seed=3)
-    with H.Harness("reference") as h:
-        h.load_full(d)
-        h.batch()
-        ref_order = h.ordering()
     ftype, fa, fb, _, _ = factor_arrays(d)
     p = HostPlan().build(d.n_nodes, ftype, fa, fb)
     assert np.array_equal(p.array("order"), ref_order)
@@ -201,14 +221,16 @@ def test_emulated_batch_matches_golden_m3500(m3500):
     assert np.abs(st - g["states"][0]).max() < 1e-7
 
 
-def test_emulated_batch_synthetic_vs_reference():
-    if not H.available("reference"):
-        pytest.skip("reference oracle not built")
-    d = datasets.manhattan_dense(600, seed=2)
-    with H.Harness("reference") as h:
-        h.load_full(d)
+def ref_emulated_batch_synthetic(impl):
+    with H.Harness(impl) as h:
+        h.load_full(datasets.manhattan_dense(600, seed=2))
         h.batch()
-        ref = h.states()
+        return {"states": h.states()}
+
+
+def test_emulated_batch_synthetic_vs_reference():
+    d = datasets.manhattan_dense(600, seed=2)
+    ref = reference("emulated_batch_synthetic__states")
     assert np.abs(emulate_batch(d) - ref).max() < 1e-6 * max(1.0, np.abs(ref).max())
 
 
@@ -471,17 +493,22 @@ def test_oracle_port_matches_golden(m3500):
         assert abs(port.chi2(m3500, st) - g["chi2"][it + 1]) < 1e-7 * g["chi2"][it + 1]
 
 
+def ref_oracle_port_small_graphs(impl):
+    out = {}
+    for n in (1, 2, 3, 11, 150):
+        with H.Harness(impl) as h:
+            h.load_full(load_m3500().head(n))
+            h.batch()
+            out[f"n{n}_states"], out[f"n{n}_chi2"] = h.states(), h.chi2()
+    return out
+
+
 def test_oracle_port_small_graphs_vs_reference(m3500):
-    if not H.available("reference"):
-        pytest.skip("reference oracle not built")
     sys.path.insert(0, ROOT)
     from oracle import port
     for n in (1, 2, 3, 11, 150):
         sub = m3500.head(n)
-        with H.Harness("reference") as h:
-            h.load_full(sub)
-            h.batch()
-            ref, c = h.states(), h.chi2()
+        ref, c = reference(f"oracle_port_small_graphs__n{n}_states"), reference(f"oracle_port_small_graphs__n{n}_chi2")
         st = port.batch_step(sub, sub.init)
         assert np.abs(st - ref).max() < 1e-9, n
         assert abs(port.chi2(sub, st) - c) <= 1e-9 * max(1.0, c)
@@ -547,21 +574,17 @@ def test_graph_file_interchange_with_reference(m3500, tmp_path):
 
 def test_reference_examples_link_unchanged(built, tmp_path):
     """SURVEY.md section 8(f) item 1: the reference's four example programs compile and link against this library
-    without a source change (only where /root/reference is present); the two that do not solve anything
-    run here on the CPU, save + load included (the upstream simple example dies in the reference's own
-    decoder because it forgets april_graph_stype_init(); this library registers the built-in types itself)."""
-    exdir = "/root/reference/examples"
-    if not os.path.isdir(exdir):
-        pytest.skip("reference sources not present")
-    libdir = os.path.join(ROOT, "aprilsam_b200", "lib")
+    without a source change (oracle/Makefile builds them into oracle/_ref/ex_* wherever it builds the reference); the
+    two that do not solve anything run here on the CPU, save + load included (the upstream simple example dies in the
+    reference's own decoder because it forgets april_graph_stype_init(); this library registers the built-in types
+    itself)."""
+    if not H.available("reference"):
+        pytest.skip("reference oracle not built")
     names = ["aprilsam_graph_save_simple", "aprilsam_graph_save_with_attributes", "aprilsam_tutorial", "aprilsam_demo"]
-    for n in names:
-        r = subprocess.run(["gcc", "-std=gnu99", "-I" + os.path.join(ROOT, "include"), "-o", str(tmp_path / n),
-                            os.path.join(exdir, n + ".c"), "-L" + libdir, "-laprilsam_b200", "-Wl,-rpath," + libdir, "-lm"],
-                           capture_output=True, text=True)
-        assert r.returncode == 0, (n, r.stderr[-2000:])
+    exe = {n: os.path.join(ROOT, "oracle", "_ref", "ex_" + n) for n in names}
+    assert all(os.path.exists(p) for p in exe.values()), "oracle/Makefile built the reference but not its examples"
     for n in names[:2]:
-        r = subprocess.run([str(tmp_path / n), "--path", str(tmp_path / (n + ".graph"))], capture_output=True, text=True, timeout=60)
+        r = subprocess.run([exe[n], "--path", str(tmp_path / (n + ".graph"))], capture_output=True, text=True, timeout=60)
         assert r.returncode == 0, (n, r.stdout[-500:], r.stderr[-500:])
         out = r.stdout
         a, b = out.split("Load graph")

@@ -1,12 +1,14 @@
 #!/usr/bin/env python
 """Generate tests/golden/*.npz from the UNMODIFIED reference (oracle/_ref, deterministic clock).
 
-Run in the build container (needs oracle/_ref built from /root/reference).  The fixtures let
-the parity tests run where the reference binary is absent.
+Needs oracle/_ref, which oracle/Makefile builds where the reference sources are present.  The
+fixtures let the parity tests run where the reference binary is absent.
   m3500_batch.npz    config 1/2: 6 consecutive april_graph_cholesky calls on the full graph
   m3500_replay.npz   config 3: demo-protocol pose-by-pose replay, chi2 / naffected / start_over
                      after every step, full state vectors at checkpoints
   tutorial.npz       the 6-pose dog-leg of examples/aprilsam_tutorial.c (incremental + batch)
+  reference_runs.npz the output of every `ref_*` driver of tests/test_host_cpu.py and
+                     tests/test_gpu_parity.py run on the reference, keys "<driver>__<name>"
 """
 import os
 import sys
@@ -75,8 +77,29 @@ def tutorial():
     print("tutorial", out["inc_chi2"], out["batch_chi2"])
 
 
+def reference_runs():
+    sys.path[:0] = [os.path.join(ROOT, "tests")]
+    import test_gpu_parity
+    import test_host_cpu
+    out = {}
+    for mod in (test_host_cpu, test_gpu_parity):
+        for name, fn in sorted(vars(mod).items()):
+            if name.startswith("ref_") and callable(fn) and name != "ref_manhattan_batch":
+                print(name, flush=True)
+                for k, v in fn("reference").items():
+                    v = np.asarray(v)
+                    if v.dtype.kind == "i" and v.size:  # orderings and counters: the smallest exact type
+                        v = v.astype(np.result_type(np.min_scalar_type(v.min()), np.min_scalar_type(v.max())))
+                    out[f"{name[4:]}__{k}"] = v
+    np.savez_compressed(os.path.join(G, "reference_runs.npz"), **out)
+
+
 if __name__ == "__main__":
+    if "--reference-runs" in sys.argv:  # only the driver outputs; the other fixtures stay as committed
+        reference_runs()
+        sys.exit(0)
     d = PoseGraphData.load(os.path.join(G, "m3500.npz"))
     m3500_batch(d)
     m3500_replay(d)
     tutorial()
+    reference_runs()

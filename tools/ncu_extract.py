@@ -5,6 +5,7 @@
     python tools/ncu_extract.py profiles/X_100k_batch_prof_raw.csv profiles/X_m3500_batch_prof_raw.csv
 """
 import csv
+import os
 import json
 import sys
 
@@ -26,6 +27,7 @@ def main():
                    "k_factor": {"bytes": int(agg.get("k_factor", 0) + agg.get("k_factor_leaf", 0)), "note": "k_factor + k_factor_leaf"},
                    "k_backsolve": {"bytes": int(agg.get("k_backsolve", 0) + agg.get("k_backsolve_leaf", 0)),
                                    "note": "k_backsolve + k_backsolve_leaf"}}
+    os.makedirs("profiles", exist_ok=True)
     json.dump(out, open("profiles/ncu_traffic.json", "w"), indent=1)
     print(json.dumps(out, indent=1))
 

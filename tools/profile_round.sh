@@ -1,5 +1,5 @@
 #!/bin/bash
-# ncu evidence for profiles/ (run under gpurun, ONE GPU): launch lists + one --set full capture of the
+# ncu launch lists and captures (ONE GPU): launch lists + one --set full capture of the
 # solve kernels for the two batch workloads.  Numbers printed by bench.py under ncu are NOT bench values.
 R=${1:-rd2}
 MODE=${2:-full}   # "launches": launch lists only

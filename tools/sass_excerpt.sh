@@ -1,9 +1,9 @@
 #!/bin/bash
-# SASS evidence for profiles/ (no GPU needed): which Blackwell/Hopper-era instructions the built library contains.
-# usage: tools/sass_excerpt.sh > profiles/rd2_sass_excerpt.txt
+# SASS evidence (no GPU needed): which Hopper-era instructions the built library contains.
+# usage: tools/sass_excerpt.sh > sass_excerpt.txt
 SO=aprilsam_b200/lib/libaprilsam_b200.so
 echo "# cuobjdump -sass $SO  ($(date -u +%F), nvcc $(nvcc --version | grep release | sed 's/.*release //'))"
-echo "# sm_100a cubin; counts of the instructions that matter (per kernel: the function the line belongs to)"
+echo "# sm_90a cubin; counts of the instructions that matter (per kernel: the function the line belongs to)"
 cuobjdump -sass $SO | awk '
 /Function :/ { fn=$3 }
 /DMMA/ { dmma[fn]++ }

@@ -1,6 +1,6 @@
 // Micro-benchmark: where the time of one 48x48 diagonal block of the team path goes (one CTA of 256 threads,
 // shared memory, clock64 stamps).  Uses the production device functions.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -I../../include -I../../aprilsam_b200/csrc -o diag_block diag_block.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -I../../include -I../../aprilsam_b200/csrc -o diag_block diag_block.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cmath>

@@ -1,5 +1,5 @@
-// Micro-benchmark: FP64 throughput of one B200 SM pipe via DFMA vs mma.sync.m8n8k4.f64 (DMMA).
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_pipes fp64_pipes.cu && ./fp64_pipes
+// Micro-benchmark: FP64 throughput of one SM pipe via DFMA vs mma.sync.m8n8k4.f64 (DMMA).
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_pipes fp64_pipes.cu && ./fp64_pipes
 #include <cstdio>
 #include <cuda_runtime.h>
 
