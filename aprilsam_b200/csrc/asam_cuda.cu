@@ -121,8 +121,6 @@ struct asam_dev {
                        // 3 mma.sync f64, operands by rows from the panel workspace (two bulk copies per tile), fused crew items
     int pb_smem = 12;  // ASAM_PB_SMEM: panel width of shared-memory fronts
     int smem_mma = 1;  // ASAM_SMEM_MMA: 0 DFMA only, 1 tensor pipe for the kept-columns update, 2 for every panel update
-    int staged = 2;    // ASAM_STAGED=0: tile mode 3 publishes the diagonal block at once; 1: in 12-column stages, the crew
-                       // polls, fetches and solves one after the other; 2: loader / solver warps in the crew (A/B)
     int solo_pb = 48;  // ASAM_SOLO_PB: staged panel width of single-CTA fronts that live in HBM
     int small_ok = 1;  // ASAM_SMALL_STEP=0 disables the fused small-step kernel (A/B measurements)
     int64_t n_small = 0;
@@ -596,8 +594,6 @@ ASAM_EXPORT int asam_dev_create(asam_dev_t **out)
         d->pb_smem = atoi(getenv("ASAM_PB_SMEM")) / 3 * 3;
     if (getenv("ASAM_SMEM_MMA"))
         d->smem_mma = atoi(getenv("ASAM_SMEM_MMA"));
-    if (getenv("ASAM_STAGED"))
-        d->staged = atoi(getenv("ASAM_STAGED"));
     if (getenv("ASAM_DIAG_MMA")) {
         const int v = atoi(getenv("ASAM_DIAG_MMA")) != 0;
         CK(cudaMemcpyToSymbol(g_diag_mma, &v, sizeof(int)));
@@ -885,7 +881,6 @@ static int launch_factor(asam_dev *d, int ntasks, const int *tasks_dev, const in
     a.spin_limit = ASAM_SPIN_LIMIT_NS;
     a.solo_pb = d->solo_pb;
     a.tile_mode = d->tile_mode;
-    a.staged = d->staged;
     a.smem_mma = d->smem_mma;
     a.pb_smem = d->pb_smem;
     a.trace = nullptr;

@@ -118,6 +118,27 @@ __device__ __forceinline__ double d_rsqrt(const double a)
 
 __device__ __forceinline__ int ld_volatile(const int *p) { return *((const volatile int *) p); }
 
+// Flags between the CTAs of a team: release on the writer's side, acquire on the reader's.  A thread that
+// publishes for its CTA does so after a barrier, which makes the release cover the writes of every thread
+// it synchronised with; a reader polls with plain volatile loads (an acquire load invalidates L1 on every poll),
+// acquires once when the value is there and barriers behind that load.  Unlike __threadfence()
+// (MEMBAR.SC.GPU + L1 invalidation on sm_90) these do not wait for a sequentially consistent order of all memory
+// operations, and they sit on the dependent chain of every panel step.
+__device__ __forceinline__ int ld_acquire(const int *p)
+{
+    int v;
+    asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_release(int *p, const int v)
+{
+    asm volatile("st.release.gpu.global.b32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ void red_release_add(int *p, const int v)
+{
+    asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+
 __device__ __forceinline__ unsigned long long d_now()
 {
     unsigned long long t;
@@ -331,7 +352,6 @@ struct FacArgs {
     int pb_smem;   // panel width of shared-memory fronts (multiple of 3)
     int smem_mma;  // shared-memory fronts on the FP64 tensor pipe: 1 = the one wide update of kept columns (incremental
                    // steps), 2 = also the 12-column panel updates, 0 = DFMA only
-    int staged;    // tile mode 3: publish L11 in 12-column stages (0: all at once)
     int tile_mode; // trailing-update tiles of the team path: 0 DFMA, 1 mma.sync f64, 2 mma.sync f64 + bulk async copies
     int solo_pb; // widest staged panel of a front that one CTA handles out of HBM (multiple of ASAM_PB)
     unsigned long long *ptrace; // optional: panel-step stamps of supernode ptrace_sn, [panel][worker < 8][8]
@@ -843,8 +863,7 @@ __device__ __forceinline__ bool team_barrier(TeamCtx &tc, int *s_flag)
 {
     __syncthreads();
     if (threadIdx.x == 0) {
-        __threadfence();
-        atomicAdd(tc.tbar_s, 1);
+        red_release_add(tc.tbar_s, 1);
         const int target = (++tc.phase) * tc.G;
         SpinClock spins;
         int ok = 1;
@@ -856,7 +875,7 @@ __device__ __forceinline__ bool team_barrier(TeamCtx &tc, int *s_flag)
                 break;
             }
         }
-        __threadfence();
+        ld_acquire(tc.tbar_s);
         *s_flag = ok;
     } else {
         tc.phase++;
@@ -1310,48 +1329,33 @@ __device__ bool team_front(const FacArgs &a, const asam_sn_desc_t &d, int s, int
             // and go to the front + the flag (8 * seq + stage); the crew solves the matching 12 columns of its rows
             // while the next sub-panel is being factored, instead of starting when all 48 are done
             constexpr int LDD = ASAM_TPB;
-            constexpr int SUB = 256; // threads that factor the block (64 threads on a two-warp barrier were SLOWER:
-                                     // the publish / update loops want the threads more than the barriers cost)
+            constexpr int SUB = 256; // threads that factor the block (one warp in registers, and 64 threads on a two-warp
+                                     // barrier, were SLOWER: the publish / update loops want the threads more than the
+                                     // barriers cost)
             int stage = 0;
-            if (tid < SUB) {
-                for (int k1 = 0; k1 < pb; k1 += ASAM_PB) {
-                    const int pbb = min(ASAM_PB, pb - k1);
-                    panel_factor(D + (size_t) k1 * LDD, LDD, k1, pbb, pb - 1, s, err, rdv, SUB);
-                    ++stage;
-                    if (a.staged) {
-                        for (int e = tid; e < pbb * pb; e += SUB) {
-                            const int j = k1 + e / pb, i = e % pb;
-                            if (i >= j)
-                                F[(k0 + i) + (size_t) (k0 + j) * ld] = D[i + j * LDD];
-                        }
-                        for (int e = tid; e < pbb; e += SUB)
-                            dinv[k0 + k1 + e] = rdv[k1 + e];
-                        bar_sub(SUB);
-                        if (tid == 0) {
-                            __threadfence();
-                            atomicExch(crew_bar, 8 * seq + stage);
-                        }
-                    }
-                    if (k1 + pbb < pb) {
-                        if (g_diag_mma)
-                            trailing_update_mma(D, LDD, D + (size_t) k1 * LDD, LDD, pbb, k1 + pbb, pb, pb - 1, SUB / 32);
-                        else
-                            trailing_update<1, 4>(D, LDD, D + (size_t) k1 * LDD, LDD, pbb, k1 + pbb, pb, pb - 1, SUB / 32);
-                        bar_sub(SUB);
-                    }
+            for (int k1 = 0; k1 < pb; k1 += ASAM_PB) {
+                const int pbb = min(ASAM_PB, pb - k1);
+                panel_factor(D + (size_t) k1 * LDD, LDD, k1, pbb, pb - 1, s, err, rdv, SUB);
+                ++stage;
+                for (int e = tid; e < pbb * pb; e += SUB) {
+                    const int j = k1 + e / pb, i = e % pb;
+                    if (i >= j)
+                        F[(k0 + i) + (size_t) (k0 + j) * ld] = D[i + j * LDD];
                 }
-            } else {
-                stage = (pb + ASAM_PB - 1) / ASAM_PB;
+                for (int e = tid; e < pbb; e += SUB)
+                    dinv[k0 + k1 + e] = rdv[k1 + e];
+                bar_sub(SUB);
+                if (tid == 0)
+                    st_release(crew_bar, 8 * seq + stage);
+                if (k1 + pbb < pb) {
+                    if (g_diag_mma)
+                        trailing_update_mma(D, LDD, D + (size_t) k1 * LDD, LDD, pbb, k1 + pbb, pb, pb - 1, SUB / 32);
+                    else
+                        trailing_update<1, 4>(D, LDD, D + (size_t) k1 * LDD, LDD, pbb, k1 + pbb, pb, pb - 1, SUB / 32);
+                    bar_sub(SUB);
+                }
             }
             __syncthreads();
-            if (!a.staged) { // (ASAM_STAGED=0, A/B: everything at once, as before)
-                writeback(k0, pb);
-                __syncthreads();
-                if (tid == 0) {
-                    __threadfence();
-                    atomicExch(crew_bar, 8 * seq + stage);
-                }
-            }
             return;
         }
         diag_factor(D, pb, rdv, s, err);
@@ -1366,95 +1370,55 @@ __device__ bool team_front(const FacArgs &a, const asam_sn_desc_t &d, int s, int
     // worker 0 has published the matching columns of L11
     auto rows_solve_staged = [&](int k0, int pb, int rb0, int seq, double *Wnext) {
         constexpr int LDD = ASAM_TPB;
-        if (a.staged >= 2 && nt == 256) {
-            // Two groups of four warps.  LOADERS (warps 4-7): wait for the flag of stage s, fetch its 12 columns of L11
-            // (one L2 round trip) into D and hand them over on named barrier 3 + s (they only arrive).  SOLVERS (warps
-            // 0-3, one row each): pick the columns up and solve.  The loaders are already polling for stage s + 1 while
-            // the solvers work on s: a stage costs the crew max(poll + fetch, solve) instead of their sum -- before,
-            // a stage took longer than the block took to publish it, the row chunks finished well after the last
-            // publish and the whole team waited for them.
-            if (tid == 0)
-                *s_flag = 1;
-            __syncthreads();
-            const int i = rb0 + tid;
-            const bool row = tid < ASAM_CROWS && i <= m;
-            int stage = 0;
-            for (int b0 = 0; b0 < pb; b0 += ASAM_PB, ++stage) {
-                const int nb = min(ASAM_PB, pb - b0);
-                if (warp >= 4) {
-                    if (tid == 128 && *s_flag) {
-                        SpinClock spins;
-                        while (ld_volatile(crew_bar) < 8 * seq + stage + 1) {
-                            __nanosleep(20);
-                            if (spin_over(spins, a.spin_limit) || ld_volatile(err) < 0) {
-                                atomicCAS(err, 0, -(1 + s));
-                                *s_flag = 0;
-                                break;
-                            }
-                        }
-                        __threadfence();
-                    }
-                    asm volatile("bar.sync 2, 128;" ::: "memory");
-                    if (*s_flag) {
-                        for (int e = tid - 128; e < nb * ASAM_TPB; e += 128) {
-                            const int j = b0 + e / ASAM_TPB, ii = e % ASAM_TPB;
-                            D[ii + j * LDD] = (ii >= j && ii < pb) ? __ldcg(&F[(k0 + ii) + (size_t) (k0 + j) * ld]) : 0.0;
-                        }
-                        if (tid - 128 < nb)
-                            rdv[b0 + tid - 128] = __ldcg(&dinv[k0 + b0 + tid - 128]);
-                    }
-                    __threadfence_block();
-                    asm volatile("bar.arrive %0, 256;" ::"r"(3 + stage) : "memory");
-                } else {
-                    asm volatile("bar.sync %0, 256;" ::"r"(3 + stage) : "memory");
-                    if (row && *s_flag)
-                        trsm_row_block(Li, D, rdv, b0, nb, F + i + (size_t) k0 * ld, ld, Wnext + (size_t) i * ASAM_LDW);
-                }
-            }
-            if (row && *s_flag)
-                for (int q = pb; q < ((pb + 3) & ~3); q++)
-                    Wnext[(size_t) i * ASAM_LDW + q] = 0.0;
-            __syncthreads();
-            return *s_flag != 0;
-        }
+        // Two groups of four warps.  LOADERS (warps 4-7): wait for the flag of stage s, fetch its 12 columns of L11
+        // (one L2 round trip) into D and hand them over on named barrier 3 + s (they only arrive).  SOLVERS (warps
+        // 0-3, one row each): pick the columns up and solve.  The loaders are already polling for stage s + 1 while
+        // the solvers work on s: a stage costs the crew max(poll + fetch, solve) instead of their sum -- before,
+        // a stage took longer than the block took to publish it, the row chunks finished well after the last
+        // publish and the whole team waited for them.
+        if (tid == 0)
+            *s_flag = 1;
         __syncthreads();
         const int i = rb0 + tid;
         const bool row = tid < ASAM_CROWS && i <= m;
         int stage = 0;
-        for (int b0 = 0; b0 < pb; b0 += ASAM_PB) {
+        for (int b0 = 0; b0 < pb; b0 += ASAM_PB, ++stage) {
             const int nb = min(ASAM_PB, pb - b0);
-            ++stage;
-            if (tid == 0) {
-                SpinClock spins;
-                int ok = 1;
-                while (ld_volatile(crew_bar) < 8 * seq + stage) {
-                    __nanosleep(20);
-                    if (spin_over(spins, a.spin_limit) || ld_volatile(err) < 0) {
-                        atomicCAS(err, 0, -(1 + s));
-                        ok = 0;
-                        break;
+            if (warp >= 4) {
+                if (tid == 128 && *s_flag) {
+                    SpinClock spins;
+                    while (ld_volatile(crew_bar) < 8 * seq + stage + 1) {
+                        __nanosleep(20);
+                        if (spin_over(spins, a.spin_limit) || ld_volatile(err) < 0) {
+                            atomicCAS(err, 0, -(1 + s));
+                            *s_flag = 0;
+                            break;
+                        }
                     }
+                    ld_acquire(crew_bar);
                 }
-                __threadfence();
-                *s_flag = ok;
+                asm volatile("bar.sync 2, 128;" ::: "memory");
+                if (*s_flag) {
+                    for (int e = tid - 128; e < nb * ASAM_TPB; e += 128) {
+                        const int j = b0 + e / ASAM_TPB, ii = e % ASAM_TPB;
+                        D[ii + j * LDD] = (ii >= j && ii < pb) ? __ldcg(&F[(k0 + ii) + (size_t) (k0 + j) * ld]) : 0.0;
+                    }
+                    if (tid - 128 < nb)
+                        rdv[b0 + tid - 128] = __ldcg(&dinv[k0 + b0 + tid - 128]);
+                }
+                __threadfence_block();
+                asm volatile("bar.arrive %0, 256;" ::"r"(3 + stage) : "memory");
+            } else {
+                asm volatile("bar.sync %0, 256;" ::"r"(3 + stage) : "memory");
+                if (row && *s_flag)
+                    trsm_row_block(Li, D, rdv, b0, nb, F + i + (size_t) k0 * ld, ld, Wnext + (size_t) i * ASAM_LDW);
             }
-            __syncthreads();
-            if (!*s_flag)
-                return false;
-            for (int e = tid; e < nb * ASAM_TPB; e += nt) {
-                const int j = b0 + e / ASAM_TPB, ii = e % ASAM_TPB;
-                D[ii + j * LDD] = (ii >= j && ii < pb) ? __ldcg(&F[(k0 + ii) + (size_t) (k0 + j) * ld]) : 0.0;
-            }
-            for (int e = tid; e < nb; e += nt)
-                rdv[b0 + e] = __ldcg(&dinv[k0 + b0 + e]);
-            __syncthreads();
-            if (row)
-                trsm_row_block(Li, D, rdv, b0, nb, F + i + (size_t) k0 * ld, ld, Wnext + (size_t) i * ASAM_LDW);
         }
-        if (row)
+        if (row && *s_flag)
             for (int q = pb; q < ((pb + 3) & ~3); q++)
                 Wnext[(size_t) i * ASAM_LDW + q] = 0.0;
-        return true;
+        __syncthreads();
+        return *s_flag != 0;
     };
     // the other crew workers: rows [rb0, rb0+ASAM_CROWS) of the panel are fetched while worker 0 factors the
     // block, then solved against the published L11
