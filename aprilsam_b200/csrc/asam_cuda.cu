@@ -551,12 +551,12 @@ ASAM_EXPORT int asam_dev_create(asam_dev_t **out)
     // launch geometry: k_factor keeps a whole front in shared memory when it fits
     int max_optin = 0;
     CK(cudaDeviceGetAttribute(&max_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-    int want = 200 * 1024; // fronts up to m = 159 stay on chip (M3500's largest is 147)
-    const char *es = getenv("ASAM_FACTOR_SMEM_KB");
-    if (es)
-        want = atoi(es) * 1024;
+    // fronts up to m = 159 stay on chip (M3500's largest is 147).  The plan decides which fronts those are with the
+    // same 200 KB (plan.c:front_fits_smem), so a device that offers less cannot run k_factor at all.
+    const int want = 200 * 1024;
     if (want > max_optin - 1024)
-        want = max_optin - 1024;
+        return set_err("k_factor needs %d KB of shared memory per block, the device offers %d KB", want / 1024,
+                       (max_optin - 1024) / 1024);
     d->fac_smem = want;
     CK(cudaFuncSetAttribute(k_factor, cudaFuncAttributeMaxDynamicSharedMemorySize, d->fac_smem));
     int occ = 0;

@@ -104,9 +104,13 @@ __device__ __forceinline__ void d_xyt_eval(const double *pa, const double *pb, c
 // 1/sqrt(a) for the Cholesky pivots: single-precision seed (MUFU.RSQ) + two Newton steps in double (relative
 // error 2^-22 -> 2^-43 -> below 2^-53; one to two ulp after rounding).  Three of these are CHAINED in every
 // 3x3 pivot block, i.e. they sit on the dependent chain of every panel of every front; the library rsqrt()
-// (MUFU.RSQ64H + a longer refinement with range fix-ups) costs about twice as much.  Pivots are O(1e-4 .. 1e7):
-// no range issue; a <= 0 gives NaN as before (and the pivot check flags it).
-__device__ __forceinline__ double d_rsqrt(const double a)
+// (MUFU.RSQ64H + a longer refinement with range fix-ups) costs about twice as much.  The float seed only exists
+// for a in the float range: information matrices carry units and the Tikhonov term may be 0, so a pivot can be
+// anywhere in the double range (every W scaled by 2^k scales every pivot by 2^k).  A pivot outside [2^-120, 2^120]
+// is brought into range by an even power of two, 4^h, and the result scaled back by 2^-h: both exact, and the
+// seed and the Newton steps scale exactly too, so a system scaled by 4^h factors to the same bits scaled.  In-range
+// pivots never take that branch; a <= 0, inf and NaN go to rsqrt() (the pivot check flags a <= 0).
+__device__ __forceinline__ double d_rsqrt_in_range(const double a)
 {
     double y = (double) rsqrtf((float) a);
     double e = fma(-a * y, y, 1.0);
@@ -114,6 +118,19 @@ __device__ __forceinline__ double d_rsqrt(const double a)
     e = fma(-a * y, y, 1.0);
     y = fma(0.5 * y, e, y);
     return y;
+}
+
+__device__ __forceinline__ double d_rsqrt(const double a)
+{
+    if (!(a >= 0x1p-120 && a <= 0x1p120)) {
+        if (!(a > 0.0 && a < INFINITY))
+            return rsqrt(a);
+        int ex;
+        frexp(a, &ex);
+        const int h = ex / 2; // a 4^-h has an exponent in {-1, 0, 1}
+        return ldexp(d_rsqrt_in_range(ldexp(a, -2 * h)), -h);
+    }
+    return d_rsqrt_in_range(a);
 }
 
 __device__ __forceinline__ int ld_volatile(const int *p) { return *((const volatile int *) p); }
@@ -2327,15 +2344,15 @@ __device__ bool cta_backsolve(const BsArgs &a, const int t, const int s, double 
                 for (int i = tid; i < n2; i += nt)
                     xf[r0 + i] = __ldcg(&a.x[3 * (size_t) d.first + r0 + i]);
                 __syncthreads();
-                // 96 rows x up to 12 columns per warp in two rounds of six: 18 loads in flight per lane (the
-                // chain of a block is this product + the triangular solve)
+                // 96 rows x ceil(bw / nwarps) columns per warp in rounds of six (two rounds with the default 8 warps):
+                // 18 loads in flight per lane (the chain of a block is this product + the triangular solve)
                 {
                     double xv[3];
 #pragma unroll
                     for (int u = 0; u < 3; u++)
                         xv[u] = lane + 32 * u < n2 ? xf[r0 + lane + 32 * u] : 0.0;
 #pragma unroll 1
-                    for (int j0 = 0; j0 < 12; j0 += 6) {
+                    for (int j0 = 0; j0 * nwarps < bw; j0 += 6) {
                         double lv[6][3];
 #pragma unroll
                         for (int j = 0; j < 6; j++) {

@@ -60,7 +60,7 @@ ASAM_API int asam_dbg_plan_append(void *p, int N, int F, const int *ftype, const
     return nt;
 }
 
-/* info: N, nsn, n_slots, ipool_n, arena_n, max_m, nnz_l_blocks, n_levels, n_factors */
+/* info: N, nsn, n_slots, ipool_n, arena_n, max_m, nnz_l_blocks, n_levels, n_factors, n_bs_leaf */
 ASAM_API void asam_dbg_plan_info(void *p, int64_t *info, double *flops)
 {
     plan_t *pl = (plan_t *) p;
@@ -73,6 +73,7 @@ ASAM_API void asam_dbg_plan_info(void *p, int64_t *info, double *flops)
     info[6] = pl->nnz_l_blocks;
     info[7] = pl->n_levels;
     info[8] = pl->n_factors;
+    info[9] = pl->n_bs_leaf;
     *flops = pl->flops;
 }
 

@@ -97,7 +97,7 @@ class HostPlan:
         a = (C.c_int64 * 16)()
         fl = C.c_double()
         self.L.asam_dbg_plan_info(self.p, a, C.byref(fl))
-        keys = ["N", "nsn", "n_slots", "ipool_n", "arena_n", "max_m", "nnz_l_blocks", "n_levels", "n_factors"]
+        keys = ["N", "nsn", "n_slots", "ipool_n", "arena_n", "max_m", "nnz_l_blocks", "n_levels", "n_factors", "n_bs_leaf"]
         d = {k: int(a[i]) for i, k in enumerate(keys)}
         d["flops"] = fl.value
         return d
