@@ -1315,7 +1315,8 @@ ASAM_EXPORT int asam_backsolve(asam_dev_t *d, int ntasks, const int32_t *btasks,
         return 1;
     if (upload(d, d->btasks_tmp.p, btasks, b))
         return 1;
-    const bool part = bfirst && !d->keep_off;
+    // (bfirst holds with ASAM_KEEP=0 too: a front re-factored whole has the same L and y in the wanted columns)
+    const bool part = bfirst != nullptr;
     if (part && upload(d, (int *) d->btasks_tmp.p + ntasks, bfirst, b))
         return 1;
     return launch_backsolve(d, ntasks, (const int *) d->btasks_tmp.p, 0, part ? (const int *) d->btasks_tmp.p + ntasks : nullptr);
@@ -1397,6 +1398,29 @@ ASAM_EXPORT int asam_debug_read_front(asam_dev_t *d, int64_t f_off, int64_t coun
 {
     CK(cudaSetDevice(d->device));
     return download(d, out, (const double *) d->arena.p + f_off, (size_t) count * sizeof(double));
+}
+
+ASAM_EXPORT int asam_debug_read_buffer(asam_dev_t *d, int id, int64_t off, int64_t bytes, void *out)
+{
+    CK(cudaSetDevice(d->device));
+    Buf *b = nullptr;
+    switch (id) {
+    case ASAM_DBG_BUF_SN: b = &d->sn; break;
+    case ASAM_DBG_BUF_IPOOL: b = &d->ipool; break;
+    case ASAM_DBG_BUF_NODE2Q: b = &d->node2q; break;
+    case ASAM_DBG_BUF_Q2NODE: b = &d->q2node; break;
+    case ASAM_DBG_BUF_FSLOT: b = &d->f_slot; break;
+    case ASAM_DBG_BUF_FTYPE: b = &d->f_type; break;
+    case ASAM_DBG_BUF_FA: b = &d->f_a; break;
+    case ASAM_DBG_BUF_FB: b = &d->f_b; break;
+    case ASAM_DBG_BUF_FZ: b = &d->f_z; break;
+    case ASAM_DBG_BUF_FW: b = &d->f_W; break;
+    default: return set_err("asam_debug_read_buffer: unknown buffer id %d", id);
+    }
+    if (off < 0 || bytes < 0 || (size_t) (off + bytes) > b->cap)
+        return set_err("asam_debug_read_buffer: [%lld, %lld) outside buffer %d of %zu bytes", (long long) off,
+                       (long long) (off + bytes), id, b->cap);
+    return download(d, out, (const char *) b->p + off, (size_t) bytes);
 }
 
 ASAM_EXPORT int asam_sync(asam_dev_t *d)

@@ -1821,6 +1821,8 @@ int plan_append(plan_t *pl, asam_dev_t *dev, int N, int n_factors, const int *ft
         }
         if (!rc && !dev)
             pl->ipool_n += seg.n;
+        if (!rc && !dev && bs_leaf_broken) /* (with a device: below, together with the device's count) */
+            pl->n_bs_leaf = 0;
         g_plan_prof[0] += pp_now() - pp_t0; /* host symbolic */
         pp_t0 = pp_now();
         if (!rc && dev) {

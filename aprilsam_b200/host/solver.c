@@ -334,6 +334,47 @@ ASAM_API double april_graph_chi2(april_graph_t *g)
     return chi2;
 }
 
+/* ---- what the last incremental call asked of the kernels (tests; asam_dbg_record_steps) ------------- */
+enum { STEP_NONE = 0, STEP_SMALL = 1, STEP_PRUNED = 2, STEP_FULL = 3, STEP_FALLBACK = 4 };
+
+typedef struct step_rec {
+    int kind, escalated, ntasks, nbt;
+    int *tasks, *nwait, *keep, *bt, *bfirst;
+    int tcap, bcap;
+} step_rec_t;
+
+static int g_record_steps = 0;
+
+static void rec_tasks(step_rec_t *r, int n, const int *tasks, const int *nwait, const int *keep)
+{
+    if (n > r->tcap) {
+        r->tcap = n + n / 2 + 16;
+        r->tasks = realloc(r->tasks, sizeof(int) * (size_t) r->tcap);
+        r->nwait = realloc(r->nwait, sizeof(int) * (size_t) r->tcap);
+        r->keep = realloc(r->keep, sizeof(int) * (size_t) r->tcap);
+    }
+    r->ntasks = n;
+    if (n > 0) {
+        memcpy(r->tasks, tasks, sizeof(int) * (size_t) n);
+        memcpy(r->nwait, nwait, sizeof(int) * (size_t) n);
+        memcpy(r->keep, keep, sizeof(int) * (size_t) n);
+    }
+}
+
+static void rec_bt(step_rec_t *r, int n, const int *bt, const int *bfirst)
+{
+    if (n > r->bcap) {
+        r->bcap = n + n / 2 + 16;
+        r->bt = realloc(r->bt, sizeof(int) * (size_t) r->bcap);
+        r->bfirst = realloc(r->bfirst, sizeof(int) * (size_t) r->bcap);
+    }
+    r->nbt = n;
+    if (n > 0) {
+        memcpy(r->bt, bt, sizeof(int) * (size_t) n);
+        memcpy(r->bfirst, bfirst, sizeof(int) * (size_t) n);
+    }
+}
+
 /* ---- solver context (hangs off param->chol) -------------------------------------------------- */
 #define SOLVER_MAGIC 0x41534d42u /* "ASMB" */
 
@@ -352,6 +393,7 @@ typedef struct solver {
     int stamp_cap, stamp_epoch;
     aprilsam_b200_escalation_fn policy; /* deterministic escalation hook (aprilsam.h) */
     void *policy_user;
+    step_rec_t rec; /* filled only while asam_dbg_record_steps is on */
 } solver_t;
 
 /* policies set before the first batch solve wait here for their solver (param -> fn) */
@@ -383,6 +425,11 @@ static void solver_destroy(solver_t *s)
     free(s->sn_stamp);
     free(s->sn_jf);
     free(s->sn_bt);
+    free(s->rec.tasks);
+    free(s->rec.nwait);
+    free(s->rec.keep);
+    free(s->rec.bt);
+    free(s->rec.bfirst);
     s->magic = 0;
     free(s);
 }
@@ -897,6 +944,11 @@ ASAM_API void april_graph_cholesky_inc(april_graph_t *graph, april_graph_cholesk
         stamp(&tp, "begin");
     }
     s->tree_fresh = 0;
+    if (g_record_steps) {
+        s->rec.kind = STEP_NONE;
+        s->rec.escalated = 0;
+        s->rec.ntasks = s->rec.nbt = 0;
+    }
     check_nodes(graph, N0, N);
     gctx_sync_factors(c, graph);
 
@@ -972,11 +1024,15 @@ ASAM_API void april_graph_cholesky_inc(april_graph_t *graph, april_graph_cholesk
     PROF_LAP(0);
     int rc = plan_append(pl, dev, N, F, c->ftype, c->fa, c->fb, marked, n_marked, &tasks, &nwait, &keep, &ntasks);
     if (rc == 2) {
+        if (g_record_steps)
+            s->rec.kind = STEP_FALLBACK;
         inc_general_fallback(graph, param, s, N, F, F0);
         goto escalate;
     }
     if (rc != 0)
         asam_fatal("april_graph_cholesky_inc: %s %s", g_error, asam_last_error());
+    if (g_record_steps)
+        rec_tasks(&s->rec, ntasks, tasks, nwait, keep);
     int policy_escalate = 0;
     if (s->policy) {
         aprilsam_b200_step_cost_t cost;
@@ -1007,6 +1063,8 @@ ASAM_API void april_graph_cholesky_inc(april_graph_t *graph, april_graph_cholesk
         int qbase = 0;
         int fstatus = 0;
         if (tr->naffected > 5) {
+            if (g_record_steps)
+                s->rec.kind = STEP_FULL;
             DEV_OK(asam_backsolve_full(dev));
             DEV_OK(asam_step_run(dev));
             DEV_OK(asam_download_x_status(dev, 0, N, x, &fstatus));
@@ -1089,6 +1147,10 @@ ASAM_API void april_graph_cholesky_inc(april_graph_t *graph, april_graph_cholesk
                 qbase = qmin;
                 DEV_OK(asam_download_x_status(dev, qbase, N - qbase, x, &fstatus));
             }
+            if (g_record_steps) {
+                s->rec.kind = small ? STEP_SMALL : STEP_PRUNED;
+                rec_bt(&s->rec, nbt, bt, bfirst);
+            }
         }
         PROF_LAP(4);
         report_factor_status(s, fstatus, "april_graph_cholesky_inc");
@@ -1125,6 +1187,8 @@ escalate:
         g_prof[10] += 1;
         param->tr->start_over = 0;
         param->tr->nlinearized_nodes = 0;
+        if (g_record_steps)
+            solver_of(param)->rec.escalated = 1;
     }
 }
 
@@ -1205,4 +1269,34 @@ ASAM_API void *asam_dbg_plan_of_param(april_graph_cholesky_param_t *param)
 {
     solver_t *s = param && param->chol ? solver_of(param) : NULL;
     return s ? (void *) &s->plan : NULL;
+}
+
+/* Step records: off by default (the solve path then only tests the flag). */
+ASAM_API void asam_dbg_record_steps(int on) { g_record_steps = on != 0; }
+
+/* The last april_graph_cholesky_inc on param: hdr = {kind (STEP_*), escalated to a batch, ntasks, nbt}; the factor
+ * task list (tasks, nwait, keep: as given to asam_factor, up to tcap) and the back-solve list (bt, bfirst: as given
+ * to asam_backsolve, up to bcap).  Returns -1 without a solver. */
+ASAM_API int asam_dbg_last_step(april_graph_cholesky_param_t *param, int *hdr, int *tasks, int *nwait, int *keep,
+                                int tcap, int *bt, int *bfirst, int bcap)
+{
+    solver_t *s = param && param->chol ? solver_of(param) : NULL;
+    if (!s)
+        return -1;
+    const step_rec_t *r = &s->rec;
+    hdr[0] = r->kind;
+    hdr[1] = r->escalated;
+    hdr[2] = r->ntasks;
+    hdr[3] = r->nbt;
+    int nt = r->ntasks < tcap ? r->ntasks : tcap, nb = r->nbt < bcap ? r->nbt : bcap;
+    if (nt > 0) {
+        memcpy(tasks, r->tasks, sizeof(int) * (size_t) nt);
+        memcpy(nwait, r->nwait, sizeof(int) * (size_t) nt);
+        memcpy(keep, r->keep, sizeof(int) * (size_t) nt);
+    }
+    if (nb > 0) {
+        memcpy(bt, r->bt, sizeof(int) * (size_t) nb);
+        memcpy(bfirst, r->bfirst, sizeof(int) * (size_t) nb);
+    }
+    return 0;
 }

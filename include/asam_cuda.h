@@ -181,6 +181,13 @@ int asam_factor_status(asam_dev_t *d, int *status_out);
 /* Debug / test access (not used on the solve path). */
 int asam_debug_read_hessian(asam_dev_t *d, int n_nodes, int n_slots, double *Adiag9, double *Aoff9, double *Bq3);
 int asam_debug_read_front(asam_dev_t *d, int64_t f_off, int64_t count, double *out);
+/* bytes [off, off+bytes) of one device mirror of host state: the plan (descriptors, int pool, node2q,
+ * q2node, factor slots) or the factor mirror (type, node ids, z, W) */
+enum {
+    ASAM_DBG_BUF_SN = 0, ASAM_DBG_BUF_IPOOL, ASAM_DBG_BUF_NODE2Q, ASAM_DBG_BUF_Q2NODE, ASAM_DBG_BUF_FSLOT,
+    ASAM_DBG_BUF_FTYPE, ASAM_DBG_BUF_FA, ASAM_DBG_BUF_FB, ASAM_DBG_BUF_FZ, ASAM_DBG_BUF_FW
+};
+int asam_debug_read_buffer(asam_dev_t *d, int id, int64_t off, int64_t bytes, void *out);
 int asam_sync(asam_dev_t *d);
 /* Counters: [0] kernel launches since creation, [1] bytes H2D, [2] bytes D2H. */
 int asam_counters(asam_dev_t *d, int64_t *out3);
