@@ -1622,6 +1622,98 @@ __device__ __forceinline__ void ticket_release(int *ticket, int *done)
     }
 }
 
+// ncol columns of 2*nr2 doubles from src (leading dim lds) to dst (leading dim ldd), both 16-byte aligned, in
+// 16-byte accesses with eight of them in flight per thread (a panel of a front in HBM to or from shared memory).
+__device__ __forceinline__ void solo_copy(double *dst, const int ldd, const double *src, const int lds, const int nr2,
+                                          const int ncol)
+{
+    const int n = nr2 * ncol, nt = blockDim.x;
+    for (int e0 = threadIdx.x; e0 < n; e0 += 8 * nt) {
+        double2 v[8];
+#pragma unroll
+        for (int u = 0; u < 8; u++) {
+            const int e = e0 + u * nt, p = e / nr2, r = e - p * nr2;
+            if (e < n)
+                v[u] = *(const double2 *) (src + 2 * r + (size_t) p * lds);
+        }
+#pragma unroll
+        for (int u = 0; u < 8; u++) {
+            const int e = e0 + u * nt, p = e / nr2, r = e - p * nr2;
+            if (e < n)
+                *(double2 *) (dst + 2 * r + (size_t) p * ldd) = v[u];
+        }
+    }
+}
+
+// Trailing update of a front in HBM by one CTA:  F[i,j] -= sum_{p<pb} P[i,p] * P[j,p]  for j in [j0, m), i in [j, m]
+// (row m = rhs).  P is the staged panel in shared memory (column p at P + p*ldp, indexed by front row, ldp = 4
+// (mod 16)).  Tiles of 32 rows x 8 columns of the lower trapezoid on the FP64 tensor pipe, dealt to the warps
+// round-robin with no barrier between them.  A warp issues the L2 loads of its NEXT tile's C before the products
+// of the current one, so their latency hides behind the tensor instructions.
+__device__ __forceinline__ void solo_tile_next(int &jb, int &ib, const int m, int n)
+{
+    for (; n > 0 && jb < m; --n) {
+        ib += 32;
+        if (ib > m) {
+            jb += 8;
+            ib = jb;
+        }
+    }
+}
+
+__device__ __noinline__ void solo_update(double *F, const int ld, const double *P, const int ldp, const int pb,
+                                         const int j0, const int m)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    const int g = lane >> 2, t = lane & 3;
+    auto load_c = [&](const int jb, const int ib, double (&v)[4][2]) {
+#pragma unroll
+        for (int mt = 0; mt < 4; mt++)
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                const int i = ib + 8 * mt + g, j = jb + 2 * t + e;
+                v[mt][e] = (jb < m && i <= m && j < m && i >= j) ? F[i + (size_t) j * ld] : 0.0;
+            }
+    };
+    int jb = j0, ib = j0;
+    solo_tile_next(jb, ib, m, warp);
+    double cv[4][2];
+    load_c(jb, ib, cv);
+    while (jb < m) {
+        int jn = jb, in = ib;
+        solo_tile_next(jn, in, m, nwarps);
+        double cn[4][2];
+        load_c(jn, in, cn);
+        double acc[4][2];
+#pragma unroll
+        for (int mt = 0; mt < 4; mt++)
+            acc[mt][0] = acc[mt][1] = 0.0;
+        const bool jok = jb + g < m;
+        for (int kk = 0; kk < pb; kk += 4) {
+            const bool kok = kk + t < pb;
+            const size_t koff = (size_t) (kk + t) * ldp;
+            const double bv = (kok && jok) ? P[(jb + g) + koff] : 0.0;
+#pragma unroll
+            for (int mt = 0; mt < 4; mt++) {
+                const int row = ib + 8 * mt + g;
+                const double av = (kok && row <= m) ? -P[row + koff] : 0.0;
+                dmma_8x8x4(acc[mt][0], acc[mt][1], av, bv);
+            }
+        }
+#pragma unroll
+        for (int mt = 0; mt < 4; mt++)
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                const int i = ib + 8 * mt + g, j = jb + 2 * t + e;
+                if (i <= m && j < m && i >= j)
+                    F[i + (size_t) j * ld] = cv[mt][e] + acc[mt][e];
+                cv[mt][e] = cn[mt][e];
+            }
+        jb = jn;
+        ib = in;
+    }
+}
+
 // One front handled by ONE CTA (the front in shared memory when it fits, else in HBM with staged
 // panels): zero + gather the Hessian entries, wait for the children of this launch, extend-add the
 // children's update matrices, eliminate the supernode's columns, publish.  t = index in the task
@@ -1649,7 +1741,7 @@ __device__ bool cta_front(const FacArgs &a, const int t, const int s, const int 
     const bool use_sm = fsz + (ld + 1) / 2 + 2 <= (long long) a.smem_doubles;
     double *F = use_sm ? sm : Fg;
     int *dmap = (int *) (sm + (use_sm ? fsz : 0)); // ld ints
-    double *Pbuf = sm + (ld + 1) / 2 + 1;           // big mode only: staged panel
+    const int pboff = ((ld + 1) / 2 + 2) & ~1;      // HBM mode: the staged panel behind dmap, 16-byte aligned
     double *dinv = a.dinv + 3 * (size_t) d.first;   // 1/L_kk of this supernode's columns
 
     // ---- 1. zero the lower trapezoid (+ rhs row), gather the original entries ---------
@@ -1847,15 +1939,17 @@ __device__ bool cta_front(const FacArgs &a, const int t, const int s, const int 
             __syncthreads();
         }
     } else {
-        // big front handled by this CTA alone: the front stays in HBM/L2, one WIDE panel (up to
-        // a.solo_pb columns, rows k0..m) at a time is staged in shared memory, factored there in
-        // 12-column sub-panels (closed-form 3x3 steps + register-tiled update of the rest of the
-        // panel), written back, and applied to the trailing matrix in one pass.  Mid-size fronts
-        // (m of a few hundred) are latency-bound on a team -- two barriers and several L2 round trips
-        // per 48 columns for a few microseconds of arithmetic -- so while the tree is wide they go
-        // through here, one SM each (host: team_size()).
-        const int avail = a.smem_doubles - ((ld + 1) / 2 + 2);
-        int PB = avail / ld;
+        // Front in HBM handled by this CTA alone (fronts whose team would be one CTA, and every such front
+        // of an incremental step): the front stays in HBM/L2; one panel of up to a.solo_pb columns, rows
+        // k0..m, is staged in shared memory, factored there in 12-column sub-panels with tensor-pipe updates
+        // between them, written back, and applied to the trailing matrix by solo_update.  Nothing else reads
+        // the front before it is published, so no flag or fence separates the steps: one CTA barrier after
+        // the staging and one after the trailing update.
+        // Staged copy: rows kr..m (kr = k0 rounded down to even) of panel column p at Pbuf[(row - kr) + p * ldp];
+        // ldp = 4 (mod 16) keeps the m8n8k4 fragment loads free of bank conflicts.  Pst addresses it by front row.
+        double *Pbuf = sm + pboff;
+        const int ldp = ((m + 2) & ~15) + (((m + 2) & 15) <= 4 ? 4 : 20);
+        int PB = (a.smem_doubles - pboff) / ldp;
         PB = PB > a.solo_pb ? a.solo_pb : PB;
         PB = PB >= ASAM_PB ? PB - (PB % ASAM_PB) : PB - (PB % 3);
         if (PB < 3) { // front too tall for even a 3-column panel (cannot happen below m ~ 8000)
@@ -1865,23 +1959,21 @@ __device__ bool cta_front(const FacArgs &a, const int t, const int s, const int 
         }
         for (int k0 = 0; k0 < c; k0 += PB) {
             const int pbw = min(PB, c - k0);
-            for (int p = warp; p < pbw; p += nwarps)
-                for (int i = k0 + lane; i <= m; i += 32)
-                    Pbuf[i + (size_t) p * ld] = F[i + (size_t) (k0 + p) * ld];
+            const int kr = k0 & ~1, nr2 = (m - kr + 2) >> 1; // staged rows kr..kr+2*nr2-1 (<= ld-1): 16-byte pairs
+            double *Pst = Pbuf - kr;
+            solo_copy(Pbuf, ldp, F + kr + (size_t) k0 * ld, ld, nr2, pbw);
             __syncthreads();
-            double *Cp = Pbuf - (size_t) k0 * ld; // the panel addressed by FRONT column index
+            double *Cp = Pst - (size_t) k0 * ldp; // the staged panel addressed by front row and FRONT column
             for (int k1 = 0; k1 < pbw; k1 += ASAM_PB) {
                 const int pb = min(ASAM_PB, pbw - k1);
-                panel_factor(Pbuf + (size_t) k1 * ld, ld, k0 + k1, pb, m, s, err, dinv);
+                panel_factor(Pst + (size_t) k1 * ldp, ldp, k0 + k1, pb, m, s, err, dinv);
                 if (k1 + pb < pbw) {
-                    trailing_update<2, 8>(Cp, ld, Pbuf + (size_t) k1 * ld, ld, pb, k0 + k1 + pb, k0 + pbw, m);
+                    trailing_update_mma(Cp, ldp, Pst + (size_t) k1 * ldp, ldp, pb, k0 + k1 + pb, k0 + pbw, m);
                     __syncthreads();
                 }
             }
-            for (int p = warp; p < pbw; p += nwarps)
-                for (int i = k0 + lane; i <= m; i += 32)
-                    F[i + (size_t) (k0 + p) * ld] = Pbuf[i + (size_t) p * ld];
-            trailing_update<4, 8>(F, ld, Pbuf, ld, pbw, k0 + pbw, m, m);
+            solo_copy(F + kr + (size_t) k0 * ld, ld, Pbuf, ldp, nr2, pbw); // L and the panel's y
+            solo_update(F, ld, Pst, ldp, pbw, k0 + pbw, m);
             __syncthreads();
         }
     }

@@ -390,10 +390,9 @@ static int front_fits_smem(int mb)
     return (int64_t) ASAM_LD(m) * m + (ASAM_LD(m) + 1) / 2 + 2 <= 25600;
 }
 
-/* Fronts up to this order that do not fit in shared memory are still handled by ONE CTA (out of
- * HBM/L2, wide staged panels: cta_front's second mode): a team pays two barriers and several L2 round
- * trips per 48 columns, which for a few hundred rows is all latency -- in the 100 k world 740 fronts of
- * order 160-300 queue for the SMs.  ASAM_SOLO_MAX_M overrides (tuning). */
+/* Fronts up to this order that do not fit in shared memory go to ONE CTA (cta_front's HBM mode) even where
+ * their team would be larger; by default (0) only the fronts whose team the level room scales below two CTAs do
+ * (build_schedule).  ASAM_SOLO_MAX_M overrides (tuning). */
 static int solo_max_m(void)
 {
     static int v = -1;
@@ -522,13 +521,18 @@ static void team_model_init(void)
         sscanf(e, "%lf,%lf,%lf,%lf,%lf", &team_model[0], &team_model[1], &team_model[2], &team_model[3], &team_model[4]);
 }
 
+/* g: the team size, 0 for one CTA on cta_front */
 static double front_lat_us(const plan_t *pl, int s, int g)
 {
     const double m = 3.0 * pl->desc[s].mb, c = 3.0 * pl->desc[s].cb;
     if (m <= 48) /* (fitted on fronts of the leaf kernel when its limit was 48) */
         return 2.0 + 0.1 * c;
-    if (front_fits_smem(pl->desc[s].mb) || g < 1)
+    if (front_fits_smem(pl->desc[s].mb))
         return 3.8 + 0.121 * m + 0.105 * c + 0.00508 * c * m;
+    if (g < 1) /* front in HBM, one CTA (cta_front): non-negative least squares over a + b m + c' c + d c m, fitted to
+                  the 816 such fronts of the 100 k world on an H100 80GB HBM3 at 400 W (tools/solo_trace.py): a = c' = 0,
+                  median error 6 %, 90th percentile 15 % */
+        return 0.119 * m + 0.00631 * c * m;
     double tiles = 0.0, crew = 0.0;
     const int npan = (int) ceil(c / 48.0);
     for (int k = 0; k < npan; k++) {
@@ -825,10 +829,11 @@ static void build_schedule(plan_t *pl)
         const char *er = getenv("ASAM_TEAM_ROOM"); /* tuning knob (tools only) */
         if (er && atoi(er) > 0)
             room = atoi(er);
-        /* smallest team: 1 (ASAM_TEAM_MIN=2 for A/B): a "team" of one CTA runs the same panel code without
-         * partners -- no idle workers while the diagonal block is factored; pays where a level holds far more
-         * team fronts than SMs (the SM time per front is what limits the level, not its latency) */
-        int gmin = 1;
+        /* A front scaled below a team of two is factored by ONE CTA on cta_front's HBM path (task word G = 0): it
+         * pays where a level holds far more team fronts than SMs (the SM time per front is what limits the level,
+         * not its latency), and one CTA needs none of the team protocol.  ASAM_TEAM_MIN=g (A/B) sets the smallest
+         * team instead; with g = 1 such fronts run the team code alone (G = 1). */
+        int gmin = 0;
         const char *em = getenv("ASAM_TEAM_MIN");
         if (em && atoi(em) >= 1)
             gmin = atoi(em);
@@ -836,10 +841,9 @@ static void build_schedule(plan_t *pl)
             int64_t w = want[pl->desc[s].level];
             if (G_of[s] > 1 && w > room) {
                 int g = (int) ((int64_t) G_of[s] * room / w);
-                G_of[s] = g < gmin ? gmin : g;
+                g = g < gmin ? gmin : g;
+                G_of[s] = g >= 2 ? g : (gmin == 1 ? -1 : 1); /* -1: one CTA, team code path */
             }
-            if (G_of[s] == 1 && !leaf[s] && !front_fits_smem(pl->desc[s].mb) && 3 * pl->desc[s].mb > solo_max_m())
-                G_of[s] = -1; /* one CTA, team code path */
         }
         free(want);
     }
@@ -852,7 +856,7 @@ static void build_schedule(plan_t *pl)
         team_model_init();
         for (int s = nsn - 1; s >= 0; s--) { /* parents have larger ids */
             const int g = G_of[s] < 0 ? 1 : G_of[s];
-            const double lat = front_lat_us(pl, s, g);
+            const double lat = front_lat_us(pl, s, G_of[s] == 1 ? 0 : g);
             lat_us[s] = lat;
             up_us[s] = lat + (pl->desc[s].parent >= 0 ? up_us[pl->desc[s].parent] : 0.0);
             if ((owner[s] == me || owner[s] == -1) && !leaf[s])
