@@ -434,9 +434,10 @@ ASAM_EXPORT int asam_step_run(asam_dev_t *d)
 // the pinned staging buffer and are fetched by the kernel itself; the recorded linearize / factor /
 // back-solve run inside that kernel; x of the back-solved supernodes (list order, 3*cb doubles each)
 // and the status word come back through pinned memory, the host spins on a sequence flag.
-// Preconditions (checked): exactly linearize + factor + backsolve recorded, no leaf kernels, every
-// factor task a single-CTA front.  Returns 2 if the step does not qualify (nothing launched; call
-// asam_step_run instead).
+// Preconditions (checked): exactly linearize + factor + backsolve recorded, no leaf kernels.  Not checked
+// here, the caller's to ensure (solver.c does): every factor task a single-CTA front -- k_step is one CTA,
+// a team task would wait for workers that never start.  Returns 2 if the step does not qualify (nothing
+// launched; call asam_step_run instead).
 ASAM_EXPORT int asam_step_small_supported(asam_dev_t *d) { return d->small_ok && !d->timing && !d->trace_on && !d->sharded; }
 
 ASAM_EXPORT int asam_step_run_small(asam_dev_t *d, double *x_out, int x_doubles, int *status_out)

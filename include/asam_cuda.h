@@ -172,8 +172,11 @@ int asam_download_x_status(asam_dev_t *d, int q_first, int q_count, double *x3, 
  * using the st mirror (april_graph.c:79-98). Deterministic reduction. */
 int asam_chi2(asam_dev_t *d, int n_factors, double *chi2_out);
 
-/* Status of the last factorisation: 0 ok, >0 = 1 + supernode id with a non-positive pivot,
- * <0 = internal dependency timeout; ASAM_STATUS_REMOTE = another rank of a sharded solve failed (the ranks agree
+/* Status of the last factorisation: 0 ok, >0 = 1 + supernode id with a non-positive (or NaN) pivot,
+ * <0 = internal dependency timeout.  A failed pivot turns its ancestors NaN, but they start only after their
+ * children have arrived, so with one failure the status names the FIRST failing supernode, never an ancestor;
+ * failures in disjoint subtrees report one of them.  A non-zero status, once read, resets the control words,
+ * so the context can factor again (tests/test_gpu_pivots.py); ASAM_STATUS_REMOTE = another rank of a sharded solve failed (the ranks agree
  * on failure before the status is read, so that all of them take the same action). */
 #define ASAM_STATUS_REMOTE (-(1 << 28))
 int asam_factor_status(asam_dev_t *d, int *status_out);
