@@ -60,6 +60,10 @@ def lib() -> C.CDLL:
     L.asam_small_step_profile.restype = None
     L.asam_dbg_profile.argtypes = [_dp, C.c_int]
     L.asam_dbg_profile.restype = None
+    L.asam_upload_loss.argtypes = [C.c_void_p, C.c_int, C.c_int, _ip, _dp]
+    L.asam_debug_read_buffer.argtypes = [C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_void_p]
+    L.asam_dbg_factor_loss.argtypes = [C.c_void_p, C.c_int, _ip, _dp]
+    L.asam_chi2.argtypes = [C.c_void_p, C.c_int, _dp]
     _lib = L
     return L
 

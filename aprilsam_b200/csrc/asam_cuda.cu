@@ -14,6 +14,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <ctime>
+#include <vector>
 
 #include "asam_cuda.h"
 
@@ -68,6 +69,8 @@ struct asam_dev {
 
     // graph mirror
     Buf f_type, f_a, f_b, f_z, f_W, f_slot;
+    Buf f_loss; // double2 {loss, k} per factor: meaningful for robust factors only; allocated at the first
+                // asam_upload_loss, so that graphs without robust factors allocate, move and read nothing more
     Buf lp, st, node2q, q2node;
     // hessian
     Buf Adiag, Aoff, Bq, y, x, dinv;
@@ -624,7 +627,7 @@ ASAM_EXPORT void asam_dev_destroy(asam_dev_t *d)
         return;
     cudaSetDevice(d->device);
     cudaStreamSynchronize(d->stream);
-    Buf *all[] = { &d->f_type, &d->f_a, &d->f_b, &d->f_z, &d->f_W, &d->f_slot, &d->lp, &d->st, &d->node2q, &d->q2node,
+    Buf *all[] = { &d->f_type, &d->f_a, &d->f_b, &d->f_z, &d->f_W, &d->f_slot, &d->f_loss, &d->lp, &d->st, &d->node2q, &d->q2node,
                    &d->Adiag, &d->Aoff, &d->Bq, &d->y, &d->x, &d->dinv, &d->sn, &d->ipool, &d->arena, &d->arrive,
                    &d->xdone, &d->xblk, &d->tbar, &d->tasks_full, &d->nwait_full, &d->btasks_full, &d->tasks_tmp, &d->nwait_tmp,
                    &d->btasks_tmp, &d->keep_tmp, &d->leaf_tasks, &d->top_tasks, &d->top_nwait, &d->ctrl, &d->partial, &d->patch_ids, &d->patch_desc, &d->pts, &d->flush, &d->trace_fac, &d->trace_bs, &d->ptrace };
@@ -665,6 +668,8 @@ ASAM_EXPORT int asam_reserve(asam_dev_t *d, int n_nodes, int n_factors, int n_sl
     rc |= buf_reserve(d, d->f_slot, Fn * sizeof(int), true, false);
     rc |= buf_reserve(d, d->f_z, Fn * 3 * sizeof(double), true, false);
     rc |= buf_reserve(d, d->f_W, Fn * 9 * sizeof(double), true, false);
+    if (d->f_loss.cap) // in use (asam_upload_loss): grows with the factor capacity
+        rc |= buf_reserve(d, d->f_loss, Fn * 2 * sizeof(double), true, false);
     rc |= buf_reserve(d, d->lp, N * 3 * sizeof(double), true, false);
     rc |= buf_reserve(d, d->st, N * 3 * sizeof(double), true, false);
     rc |= buf_reserve(d, d->node2q, N * sizeof(int), true, false);
@@ -700,6 +705,24 @@ ASAM_EXPORT int asam_upload_factors(asam_dev_t *d, int first, int count, const i
     rc |= upload(d, (double *) d->f_z.p + 3 * (size_t) first, z3, count * 3 * sizeof(double));
     rc |= upload(d, (double *) d->f_W.p + 9 * (size_t) first, W9, count * 9 * sizeof(double));
     return rc;
+}
+
+ASAM_EXPORT int asam_upload_loss(asam_dev_t *d, int first, int count, const int32_t *loss, const double *k)
+{
+    if (count <= 0)
+        return 0;
+    if (((size_t) first + count) * sizeof(int) > d->f_type.cap)
+        return set_err("asam_upload_loss: capacity (call asam_reserve)");
+    // first robust factor of this context: one record per factor of the reserved capacity
+    if (buf_reserve(d, d->f_loss, d->f_type.cap / sizeof(int) * 2 * sizeof(double), true, false))
+        return 1;
+    // one 16-byte record per factor: the loss code travels as a double next to k
+    std::vector<double> rec(2 * (size_t) count);
+    for (int i = 0; i < count; i++) {
+        rec[2 * (size_t) i] = (double) loss[i];
+        rec[2 * (size_t) i + 1] = k[i];
+    }
+    return upload(d, (double *) d->f_loss.p + 2 * (size_t) first, rec.data(), rec.size() * sizeof(double));
 }
 
 ASAM_EXPORT int asam_upload_points(asam_dev_t *d, int which, int first, int count, const double *p3)
@@ -831,6 +854,7 @@ ASAM_EXPORT int asam_linearize(asam_dev_t *d, int f_first, int f_count, const do
     a.f_slot = (const int *) d->f_slot.p;
     a.f_z = (const double *) d->f_z.p;
     a.f_W = (const double *) d->f_W.p;
+    a.f_loss = (const double2 *) d->f_loss.p;
     a.lp = (const double *) d->lp.p;
     a.st = (const double *) d->st.p;
     a.pts = nullptr;
@@ -1349,8 +1373,8 @@ ASAM_EXPORT int asam_chi2(asam_dev_t *d, int n_factors, double *chi2_out)
         return 1;
     k_chi2_partial<<<nblk, 256, 0, d->stream>>>((const int *) d->f_type.p, (const int *) d->f_a.p,
                                                  (const int *) d->f_b.p, (const double *) d->f_z.p,
-                                                 (const double *) d->f_W.p, (const double *) d->st.p, n_factors,
-                                                 partial + 1);
+                                                 (const double *) d->f_W.p, (const double2 *) d->f_loss.p,
+                                                 (const double *) d->st.p, n_factors, partial + 1);
     k_chi2_final<<<1, 256, 0, d->stream>>>(partial + 1, nblk, partial);
     d->n_launch += 2;
     CK(cudaGetLastError());
@@ -1416,6 +1440,7 @@ ASAM_EXPORT int asam_debug_read_buffer(asam_dev_t *d, int id, int64_t off, int64
     case ASAM_DBG_BUF_FB: b = &d->f_b; break;
     case ASAM_DBG_BUF_FZ: b = &d->f_z; break;
     case ASAM_DBG_BUF_FW: b = &d->f_W; break;
+    case ASAM_DBG_BUF_FLOSS: b = &d->f_loss; break;
     default: return set_err("asam_debug_read_buffer: unknown buffer id %d", id);
     }
     if (off < 0 || bytes < 0 || (size_t) (off + bytes) > b->cap)

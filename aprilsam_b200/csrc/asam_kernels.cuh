@@ -1,7 +1,8 @@
 // asam_kernels.cuh -- device code of the AprilSAM Gauss-Newton path for sm_90a (H100).
 //
 //   k_linearize   one thread per factor: residual, Jacobians, J'WJ / J'Wr, atomically
-//                 scattered into the block Hessian (Adiag / Aoff / Bq).
+//                 scattered into the block Hessian (Adiag / Aoff / Bq).  Robust xyt factors (type 32)
+//                 scale W by their IRLS weight at the residual first.
 //                 reference: april_graph_xyt.c:62-124, april_graph_xytpos.c:63-102,
 //                            aprilsam.c:154-195 (batch), :508-542 (incremental)
 //   k_factor      persistent, dependency-driven multifrontal supernodal Cholesky with the
@@ -101,6 +102,28 @@ __device__ __forceinline__ void d_xyt_eval(const double *pa, const double *pb, c
     r[2] = d_mod2pi(z[2] - zh2);
 }
 
+// Factor types (aprilsam.h): 1 xyt, 2 xytpos prior, 32 xyt with a robust loss.  Types 1 and 32 have the
+// same two poses, Jacobians and residual; the loss only scales W.
+__device__ __forceinline__ bool d_two_pose(const int type) { return type == 1 || type == 32; }
+
+// Robust loss of a type-32 factor at s = r'Wr (loss 1 Huber, 2 Cauchy; k > 0 and finite, checked on the
+// host): the IRLS weight w = rho'(s) and the cost rho(s).  A NaN s gives NaN for both.
+__device__ __forceinline__ double d_loss_weight(const int loss, const double k, const double s)
+{
+    const double k2 = k * k;
+    if (loss == 1)
+        return s <= k2 ? 1.0 : k / sqrt(s);
+    return 1.0 / (1.0 + s / k2);
+}
+
+__device__ __forceinline__ double d_loss_rho(const int loss, const double k, const double s)
+{
+    const double k2 = k * k;
+    if (loss == 1)
+        return s <= k2 ? s : 2.0 * k * sqrt(s) - k2;
+    return k2 * log1p(s / k2);
+}
+
 // 1/sqrt(a) for the Cholesky pivots: single-precision seed (MUFU.RSQ) + two Newton steps in double (relative
 // error 2^-22 -> 2^-43 -> below 2^-53; one to two ulp after rounding).  Three of these are CHAINED in every
 // 3x3 pivot block, i.e. they sit on the dependent chain of every panel of every front; the library rsqrt()
@@ -194,6 +217,7 @@ __device__ __forceinline__ bool spin_over(SpinClock &c, long long limit_ns)
 struct LinArgs {
     const int *f_type, *f_a, *f_b, *f_slot;
     const double *f_z, *f_W;
+    const double2 *f_loss; // {loss, k} per factor; read by robust factors (type 32) only
     const double *lp, *st;
     const double *pts; // optional, indexed from f_first
     const int *node2q;
@@ -208,7 +232,7 @@ __device__ __forceinline__ void linearize_body(const LinArgs &a, const int t)
     const int f = a.f_first + (live ? t : 0);
     const int type = live ? a.f_type[f] : 0;
     const int na = live ? a.f_a[f] : -1;
-    const int nb = (live && type == 1) ? a.f_b[f] : -1;
+    const int nb = (live && d_two_pose(type)) ? a.f_b[f] : -1;
     double z[3], W[9];
 #pragma unroll
     for (int i = 0; i < 3; i++)
@@ -226,7 +250,7 @@ __device__ __forceinline__ void linearize_body(const LinArgs &a, const int t)
         // J'W = W ; (J'W) J = W ; keep scalar row <= col  (aprilsam.c:171-172)
         ca9[0] = W[0]; ca9[1] = W[1]; ca9[2] = W[2]; ca9[3] = W[4]; ca9[4] = W[5]; ca9[5] = W[8];
         d_av(W, r, ca9 + 6);
-    } else if (live) { // xyt factor
+    } else if (live) { // xyt factor (type 1 or 32)
         const int qa = a.node2q[na], qb = a.node2q[nb];
         double pa[3], pb[3];
         if (a.pts) {
@@ -239,6 +263,15 @@ __device__ __forceinline__ void linearize_body(const LinArgs &a, const int t)
         }
         double Ja[9], Jb[9], r[3], JatW[9], JbtW[9], D[9];
         d_xyt_eval(pa, pb, z, Ja, Jb, r);
+        if (type == 32) { // robust: IRLS weight at r, W_eff = w W (no second-order term: stays PSD)
+            const double2 lk = a.f_loss[f];
+            double X[3];
+            d_av(W, r, X);
+            const double w = d_loss_weight((int) lk.x, lk.y, r[0] * X[0] + r[1] * X[1] + r[2] * X[2]);
+#pragma unroll
+            for (int i = 0; i < 9; i++)
+                W[i] *= w;
+        }
         d_atb(Ja, W, JatW); // J_a' W
         d_atb(Jb, W, JbtW); // J_b' W
         // diagonal blocks: entries with scalar row <= col only (aprilsam.c:171-172)
@@ -2832,8 +2865,8 @@ __global__ void __launch_bounds__(256, 1) k_step(StepArgs a)
 // chi2
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_chi2_partial(const int *f_type, const int *f_a, const int *f_b,
-                                                      const double *f_z, const double *f_W, const double *st,
-                                                      int n_factors, double *partial)
+                                                      const double *f_z, const double *f_W, const double2 *f_loss,
+                                                      const double *st, int n_factors, double *partial)
 {
     __shared__ double red[256];
     int f = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2849,7 +2882,7 @@ __global__ void __launch_bounds__(256) k_chi2_partial(const int *f_type, const i
         for (int i = 0; i < 9; i++)
             W[i] = f_W[9 * (size_t) f + i];
         double scale;
-        if (type == 1) { // xyt at `state`, weight 0.5   (april_graph.c:86-89)
+        if (d_two_pose(type)) { // xyt at `state`, weight 0.5   (april_graph.c:86-89)
             int nb = f_b[f];
             double pa[3], pb[3], Ja[9], Jb[9];
 #pragma unroll
@@ -2864,7 +2897,13 @@ __global__ void __launch_bounds__(256) k_chi2_partial(const int *f_type, const i
         }
         double X[3];
         d_av(W, r, X);
-        v = scale * (r[0] * X[0] + r[1] * X[1] + r[2] * X[2]);
+        const double s = r[0] * X[0] + r[1] * X[1] + r[2] * X[2];
+        if (type == 32) { // robust xyt: 0.5 rho(s)
+            const double2 lk = f_loss[f];
+            v = scale * d_loss_rho((int) lk.x, lk.y, s);
+        } else {
+            v = scale * s;
+        }
     }
     red[threadIdx.x] = v;
     __syncthreads();

@@ -59,6 +59,18 @@ def _load(impl: str) -> C.CDLL:
     lib.h_add_node.argtypes = [C.c_void_p, _dp]
     lib.h_add_xyt.argtypes = [C.c_void_p, C.c_int, C.c_int, _dp, _dp]
     lib.h_add_xytpos.argtypes = [C.c_void_p, C.c_int, _dp, _dp]
+    # entry points added with robust factors: a prebuilt reference harness (oracle/_ref/, kept where the reference
+    # sources are absent) may predate them, and the reference flavours never call them
+    for name, args in (("h_add_xyt_robust", [C.c_void_p, C.c_int, C.c_int, _dp, _dp, C.c_int, C.c_double]),
+                       ("h_set_loss", [C.c_void_p, C.c_int, C.c_int, C.c_double]),
+                       ("h_set_scan_loss", [C.c_void_p, C.c_int, C.c_double]),
+                       ("h_eval", [C.c_void_p, C.c_int, C.c_int, _dp]),
+                       ("h_copy_factor", [C.c_void_p, C.c_int]),
+                       ("h_dof", [C.c_void_p])):
+        if hasattr(lib, name):
+            getattr(lib, name).argtypes = args
+        elif impl == "b200":
+            raise AttributeError(f"{path}: {name} missing - rebuild with aprilsam_b200.build")
     lib.h_relinearize.argtypes = [C.c_void_p, C.c_int]
     lib.h_get.argtypes = [C.c_void_p, C.c_int, _dp]
     lib.h_set.argtypes = [C.c_void_p, C.c_int, _dp]
@@ -179,6 +191,38 @@ class Harness:
         z = np.ascontiguousarray(z, dtype=np.float64)
         W = np.ascontiguousarray(W, dtype=np.float64).reshape(9)
         return self.lib.h_add_xytpos(self.h, a, _d(z), _d(W))
+
+    # robust loop closures (aprilsam_b200 extension: the reference build returns -1 / ignores them)
+    HUBER, CAUCHY = 1, 2
+
+    def add_xyt_robust(self, a: int, b: int, z, W, loss: int, k: float) -> int:
+        """aprilsam_b200_factor_xyt_robust_create + append; -1 (no factor) for an invalid loss / k."""
+        z = np.ascontiguousarray(z, dtype=np.float64)
+        W = np.ascontiguousarray(W, dtype=np.float64).reshape(9)
+        return self.lib.h_add_xyt_robust(self.h, a, b, _d(z), _d(W), int(loss), float(k))
+
+    def set_loss(self, idx: int, loss: int, k: float) -> int:
+        """aprilsam_b200_factor_set_loss on factor idx: 0 ok, -1 otherwise."""
+        return self.lib.h_set_loss(self.h, idx, int(loss), float(k))
+
+    def set_scan_loss(self, loss: int, k: float = 0.0) -> None:
+        """replay_to / load_full create every scan edge (|a - b| != 1) as a robust factor; loss 0 = plain xyt."""
+        self.lib.h_set_scan_loss(self.h, int(loss), float(k))
+
+    def eval(self, idx: int, at_state: bool = False):
+        """The factor's eval (l_point) or state_eval (state) hook -> (r, J0, J1, W, chi2), None if unset."""
+        out = np.zeros(31, dtype=np.float64)
+        if self.lib.h_eval(self.h, idx, int(at_state), _d(out)) < 0:
+            return None
+        return out[:3].copy(), out[3:12].reshape(3, 3).copy(), out[12:21].reshape(3, 3).copy(), \
+            out[21:30].reshape(3, 3).copy(), float(out[30])
+
+    def copy_factor(self, idx: int) -> int:
+        """Append factor->copy(factor); returns the new index."""
+        return self.lib.h_copy_factor(self.h, idx)
+
+    def dof(self) -> int:
+        return self.lib.h_dof(self.h)
 
     def relinearize(self, i: int):
         self.lib.h_relinearize(self.h, i)

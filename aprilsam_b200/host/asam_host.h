@@ -12,6 +12,13 @@
 
 #define ASAM_API __attribute__((visibility("default")))
 
+/* Factor types the solver treats as an xyt factor between two poses: plain xyt (1) and robust xyt (32).
+ * Every host site that decides "one pose or two" asks this, never the type code itself. */
+static inline int asam_two_pose_type(int type)
+{
+    return type == APRIL_GRAPH_FACTOR_XYT_TYPE || type == APRIL_GRAPH_FACTOR_XYT_ROBUST_TYPE;
+}
+
 /* ---- small containers ---------------------------------------------------------------- */
 typedef struct {
     int *p;
@@ -162,9 +169,11 @@ void plan_work(const plan_t *pl, const int *tasks, int ntasks, double *step_work
 
 /* ---- solver context (solver.c) --------------------------------------------------------- */
 void asam_graph_forget(april_graph_t *g);
+/* graph.c: loss code and k of a factor; (0, 0) for factors without a robust loss */
+void asam_factor_loss(const april_graph_factor_t *f, int32_t *loss, double *k);
 /* serial.c */
 extern const stype_t stype_april_graph, stype_april_graph_attr, stype_april_node_xyt, stype_april_factor_xyt,
-    stype_april_factor_xytpos;
+    stype_april_factor_xytpos, stype_april_factor_xyt_robust;
 april_graph_attr_t *asam_attr_dup(const april_graph_attr_t *a);
 void asam_set_error(const char *fmt, ...);
 void asam_fatal(const char *fmt, ...);

@@ -24,6 +24,17 @@ ASAM_API int asam_dbg_plan_build(void *p, int N, int F, const int *ftype, const 
     return plan_build((plan_t *) p, NULL, N, F, ftype, fa, fb);
 }
 
+/* type of factor idx of g, and its loss code / k ((0, 0) without a robust loss) */
+ASAM_API int asam_dbg_factor_loss(april_graph_t *g, int idx, int *loss, double *k)
+{
+    april_graph_factor_t *f;
+    zarray_get(g->factors, idx, &f);
+    int32_t l;
+    asam_factor_loss(f, &l, k);
+    *loss = l;
+    return f->type;
+}
+
 /* multi-GPU schedule of rank `rank` of `world` (no device, no communicator needed) */
 ASAM_API int asam_dbg_plan_build_sharded(void *p, int world, int rank, int N, int F, const int *ftype, const int *fa,
                                          const int *fb)

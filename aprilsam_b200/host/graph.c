@@ -274,6 +274,113 @@ ASAM_API april_graph_factor_t *april_graph_factor_xyt_create(int a, int b, const
     return f;
 }
 
+/* ---- robust xyt factor (extension, aprilsam.h): xyt + a loss the factor owns behind u.common.impl ---- */
+typedef struct {
+    int loss;
+    double k;
+} robust_loss_t;
+
+static int loss_valid(int loss, double k)
+{
+    if (loss != APRILSAM_B200_LOSS_HUBER && loss != APRILSAM_B200_LOSS_CAUCHY) {
+        asam_set_error("robust loss %d: expected %d (Huber) or %d (Cauchy)", loss, APRILSAM_B200_LOSS_HUBER,
+                       APRILSAM_B200_LOSS_CAUCHY);
+        return 0;
+    }
+    if (!(k > 0.0) || !isfinite(k)) {
+        asam_set_error("robust loss scale k = %g: must be finite and > 0", k);
+        return 0;
+    }
+    return 1;
+}
+
+void asam_factor_loss(const april_graph_factor_t *f, int32_t *loss, double *k)
+{
+    const robust_loss_t *r = f->type == APRIL_GRAPH_FACTOR_XYT_ROBUST_TYPE ? f->u.common.impl : NULL;
+    *loss = r ? r->loss : 0;
+    *k = r ? r->k : 0.0;
+}
+
+/* xyt evaluation -> W_eff = w W and chi2 = rho(s), s = r'Wr as eval_finish left it in chi2 (the same
+ * arithmetic as k_linearize / k_chi2_partial) */
+static april_graph_factor_eval_t *robust_weigh(const april_graph_factor_t *f, april_graph_factor_eval_t *ev)
+{
+    const robust_loss_t *r = f->u.common.impl;
+    const double s = ev->chi2, k2 = r->k * r->k;
+    double w, rho;
+    if (r->loss == APRILSAM_B200_LOSS_HUBER) {
+        w = s <= k2 ? 1.0 : r->k / sqrt(s);
+        rho = s <= k2 ? s : 2.0 * r->k * sqrt(s) - k2;
+    } else {
+        w = 1.0 / (1.0 + s / k2);
+        rho = k2 * log1p(s / k2);
+    }
+    for (int i = 0; i < 9; i++)
+        ev->W->data[i] *= w;
+    ev->chi2 = rho;
+    return ev;
+}
+
+static april_graph_factor_eval_t *robust_eval(april_graph_factor_t *f, april_graph_t *g, april_graph_factor_eval_t *ev)
+{
+    return robust_weigh(f, xyt_eval(f, g, ev));
+}
+
+static april_graph_factor_eval_t *robust_state_eval(april_graph_factor_t *f, april_graph_t *g,
+                                                    april_graph_factor_eval_t *ev)
+{
+    return robust_weigh(f, xyt_state_eval(f, g, ev));
+}
+
+static void robust_destroy(april_graph_factor_t *f)
+{
+    free(f->u.common.impl);
+    factor_common_destroy(f);
+}
+
+static april_graph_factor_t *robust_copy(april_graph_factor_t *f)
+{
+    const robust_loss_t *r = f->u.common.impl;
+    april_graph_factor_t *c = aprilsam_b200_factor_xyt_robust_create(f->nodes[0], f->nodes[1], f->u.common.z,
+                                                                     f->u.common.ztruth, f->u.common.W, r->loss, r->k);
+    c->attr = asam_attr_dup(f->attr);
+    return c;
+}
+
+ASAM_API april_graph_factor_t *aprilsam_b200_factor_xyt_robust_create(int a, int b, const double *z,
+                                                                     const double *ztruth, const matd_t *W, int loss,
+                                                                     double k)
+{
+    if (!loss_valid(loss, k))
+        return NULL;
+    april_graph_factor_t *f = april_graph_factor_xyt_create(a, b, z, ztruth, W);
+    robust_loss_t *r = malloc(sizeof(*r));
+    r->loss = loss;
+    r->k = k;
+    f->type = APRIL_GRAPH_FACTOR_XYT_ROBUST_TYPE;
+    f->u.common.impl = r;
+    f->copy = robust_copy;
+    f->eval = robust_eval;
+    f->state_eval = robust_state_eval;
+    f->destroy = robust_destroy;
+    f->stype = &stype_april_factor_xyt_robust;
+    return f;
+}
+
+ASAM_API int aprilsam_b200_factor_set_loss(april_graph_factor_t *f, int loss, double k)
+{
+    if (!f || f->type != APRIL_GRAPH_FACTOR_XYT_ROBUST_TYPE || !f->u.common.impl) {
+        asam_set_error("aprilsam_b200_factor_set_loss: factor of type %d has no robust loss", f ? f->type : -1);
+        return -1;
+    }
+    if (!loss_valid(loss, k))
+        return -1;
+    robust_loss_t *r = f->u.common.impl;
+    r->loss = loss;
+    r->k = k;
+    return 0;
+}
+
 static april_graph_factor_eval_t *xytpos_eval(april_graph_factor_t *f, april_graph_t *g, april_graph_factor_eval_t *ev)
 {
     if (!ev)

@@ -1077,7 +1077,7 @@ static int plan_build_impl(plan_t *pl, asam_dev_t *dev, int N, int n_factors, co
     pairmap_init(&pl->pairs, n_factors);
     ivec_t plo = { 0 }, phi = { 0 };
     for (int f = 0; f < n_factors; f++) {
-        if (ftype[f] == APRIL_GRAPH_FACTOR_XYT_TYPE) {
+        if (asam_two_pose_type(ftype[f])) {
             int a = fa[f], b = fb[f];
             if (a == b || a < 0 || b < 0 || a >= N || b >= N) {
                 asam_set_error("factor %d: bad node ids (%d,%d)", f, a, b);
@@ -1503,7 +1503,7 @@ int plan_append(plan_t *pl, asam_dev_t *dev, int N, int n_factors, const int *ft
         *keep_out = NULL;
     *ntasks_out = 0;
     for (int f = F0; f < n_factors; f++) {
-        if (ftype[f] == APRIL_GRAPH_FACTOR_XYT_TYPE) {
+        if (asam_two_pose_type(ftype[f])) {
             if (fa[f] == fb[f] || fa[f] < 0 || fb[f] < 0 || fa[f] >= N || fb[f] >= N) {
                 asam_set_error("factor %d: bad node ids (%d,%d)", f, fa[f], fb[f]);
                 return 1;
@@ -1565,7 +1565,7 @@ int plan_append(plan_t *pl, asam_dev_t *dev, int N, int n_factors, const int *ft
     const int slot0 = pl->n_slots;
     ivec_t nlo = { 0 }, nhi = { 0 };
     for (int f = F0; f < n_factors; f++) {
-        if (ftype[f] != APRIL_GRAPH_FACTOR_XYT_TYPE) {
+        if (!asam_two_pose_type(ftype[f])) {
             pl->fslot[f] = -1;
             continue;
         }

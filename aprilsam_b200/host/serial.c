@@ -476,8 +476,12 @@ static void *node_xyt_decode(const stype_t *st, const uint8_t *data, uint32_t *p
     return n;
 }
 
-static void factor_common_encode(uint8_t *data, uint32_t *pos, const april_graph_factor_t *f)
+/* xyt / xytpos: node ids | z | ztruth | W | attr.  The robust xyt factor (this library's own type) puts
+ * u32 loss | f64 k between W and attr. */
+static void factor_encode(const stype_t *st, uint8_t *data, uint32_t *pos, const void *obj)
 {
+    (void) st;
+    const april_graph_factor_t *f = obj;
     for (int i = 0; i < f->nnodes; i++)
         encode_u32(data, pos, (uint32_t) f->nodes[i]);
     for (int i = 0; i < 3; i++)
@@ -485,18 +489,20 @@ static void factor_common_encode(uint8_t *data, uint32_t *pos, const april_graph
     opt3_encode(data, pos, f->u.common.ztruth);
     for (int i = 0; i < 9; i++)
         encode_f64(data, pos, f->u.common.W->data[i]);
+    if (f->type == APRIL_GRAPH_FACTOR_XYT_ROBUST_TYPE) {
+        int32_t loss;
+        double k;
+        asam_factor_loss(f, &loss, &k);
+        encode_u32(data, pos, (uint32_t) loss);
+        encode_f64(data, pos, k);
+    }
     attr_of_encode(data, pos, f->attr);
-}
-
-static void factor_encode(const stype_t *st, uint8_t *data, uint32_t *pos, const void *obj)
-{
-    (void) st;
-    factor_common_encode(data, pos, (const april_graph_factor_t *) obj);
 }
 
 static void *factor_decode(const stype_t *st, const uint8_t *data, uint32_t *pos, uint32_t len)
 {
-    const int binary = !strcmp(st->name, "april_graph_factor_xyt");
+    const int robust = st == &stype_april_factor_xyt_robust;
+    const int binary = robust || !strcmp(st->name, "april_graph_factor_xyt");
     int a = (int) decode_u32(data, pos, len), b = binary ? (int) decode_u32(data, pos, len) : -1;
     double z[3], zt[3];
     for (int i = 0; i < 3; i++)
@@ -505,8 +511,17 @@ static void *factor_decode(const stype_t *st, const uint8_t *data, uint32_t *pos
     matd_t *W = matd_create(3, 3);
     for (int i = 0; i < 9; i++)
         W->data[i] = decode_f64(data, pos, len);
-    april_graph_factor_t *f = binary ? april_graph_factor_xyt_create(a, b, z, ht ? zt : NULL, W)
-                                     : april_graph_factor_xytpos_create(a, z, ht ? zt : NULL, W);
+    april_graph_factor_t *f;
+    if (robust) {
+        int loss = (int) decode_u32(data, pos, len);
+        double k = decode_f64(data, pos, len);
+        f = aprilsam_b200_factor_xyt_robust_create(a, b, z, ht ? zt : NULL, W, loss, k);
+        if (!f)
+            asam_fatal("graph file: robust factor %d-%d: %s", a, b, aprilsam_b200_last_error());
+    } else {
+        f = binary ? april_graph_factor_xyt_create(a, b, z, ht ? zt : NULL, W)
+                   : april_graph_factor_xytpos_create(a, z, ht ? zt : NULL, W);
+    }
     f->attr = stype_decode_object(data, pos, len, NULL);
     matd_destroy(W);
     return f;
@@ -518,6 +533,8 @@ ASAM_API const stype_t stype_april_factor_xyt = { .name = "april_graph_factor_xy
                                                   .decode = factor_decode };
 ASAM_API const stype_t stype_april_factor_xytpos = { .name = "april_graph_factor_xytpos", .encode = factor_encode,
                                                      .decode = factor_decode };
+ASAM_API const stype_t stype_april_factor_xyt_robust = { .name = "april_graph_factor_xyt_robust",
+                                                         .encode = factor_encode, .decode = factor_decode };
 
 /* ---- graph codec + files (april_graph.c:250-326, :377-426) ---------------------------------------- */
 static void graph_encode(const stype_t *st, uint8_t *data, uint32_t *pos, const void *obj)
@@ -571,6 +588,7 @@ ASAM_API void april_graph_stype_init(void)
     stype_register(&stype_april_node_xyt);
     stype_register(&stype_april_factor_xyt);
     stype_register(&stype_april_factor_xytpos);
+    stype_register(&stype_april_factor_xyt_robust);
 }
 
 /* returns 1 on success, 0 on failure (april_graph.c:377-398) */

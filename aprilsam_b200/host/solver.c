@@ -126,6 +126,8 @@ typedef struct gctx {
     int nf_dev; /* factors mirrored in HBM */
     int *ftype, *fa, *fb;
     double *zw; /* host mirror of what HBM holds: 12 doubles per factor (z[3], W[9]) */
+    int32_t *floss; /* loss code and k per factor (0 / 0 without a robust loss); in HBM for robust factors */
+    double *fk;
     int fcap;
     double *stage; /* host staging for poses */
     int stage_cap;
@@ -173,6 +175,8 @@ static void gctx_unref(gctx_t *c)
         }
     pthread_mutex_unlock(&g_ctx_lock);
     free(c->zw);
+    free(c->floss);
+    free(c->fk);
     asam_dev_destroy(c->dev);
     free(c->ftype);
     free(c->fa);
@@ -229,24 +233,32 @@ static void gctx_sync_factors(gctx_t *c, april_graph_t *g)
         c->fa = realloc(c->fa, sizeof(int) * (size_t) c->fcap);
         c->fb = realloc(c->fb, sizeof(int) * (size_t) c->fcap);
         c->zw = realloc(c->zw, sizeof(double) * 12 * (size_t) c->fcap);
+        c->floss = realloc(c->floss, sizeof(int32_t) * (size_t) c->fcap);
+        c->fk = realloc(c->fk, sizeof(double) * (size_t) c->fcap);
     }
     int first = c->nf_dev, cnt = F - first;
     double *zw = malloc(sizeof(double) * 12 * (size_t) cnt);
     double *z = zw, *W = zw + 3 * (size_t) cnt;
+    int robust = 0;
     for (int k = 0; k < cnt; k++) {
         april_graph_factor_t *f = factor_at(g, first + k);
         int i = first + k;
-        if (f->type == APRIL_GRAPH_FACTOR_XYT_TYPE && f->nnodes == 2) {
+        if (asam_two_pose_type(f->type) && f->nnodes == 2) {
             c->fa[i] = f->nodes[0];
             c->fb[i] = f->nodes[1];
         } else if (f->type == APRIL_GRAPH_FACTOR_XYTPOS_TYPE && f->nnodes == 1) {
             c->fa[i] = f->nodes[0];
             c->fb[i] = -1;
         } else {
-            asam_fatal("factor %d has type %d / %d nodes: only xyt (1) and xytpos (2) factors are supported", i,
-                       f->type, f->nnodes);
+            asam_fatal("factor %d has type %d / %d nodes: only xyt (1), xytpos (2) and robust xyt (32) factors are "
+                       "supported", i, f->type, f->nnodes);
         }
         c->ftype[i] = f->type;
+        asam_factor_loss(f, &c->floss[i], &c->fk[i]);
+        if (f->type == APRIL_GRAPH_FACTOR_XYT_ROBUST_TYPE && !c->floss[i])
+            asam_fatal("factor %d: robust xyt factor without a loss (create it with "
+                       "aprilsam_b200_factor_xyt_robust_create)", i);
+        robust |= c->floss[i] != 0;
         const matd_t *Wm = f->u.common.W;
         if (!Wm || Wm->nrows != 3 || Wm->ncols != 3 || !f->u.common.z)
             asam_fatal("factor %d: W must be 3x3 and z non-NULL", i);
@@ -260,12 +272,15 @@ static void gctx_sync_factors(gctx_t *c, april_graph_t *g)
     }
     DEV_OK(asam_reserve(c->dev, N + 64, F + F / 4 + 64, 0, 0, 0, 0));
     DEV_OK(asam_upload_factors(c->dev, first, cnt, c->ftype + first, c->fa + first, c->fb + first, z, W));
+    if (robust) /* graphs without robust factors never move loss records */
+        DEV_OK(asam_upload_loss(c->dev, first, cnt, c->floss + first, c->fk + first));
     free(zw);
     c->nf_dev = F;
 }
 
 /* The reference reads every factor on every batch call (aprilsam.c:154-195), so a caller may edit
- * z / W in place between calls (re-weighting, robust kernels) or swap a factor for another one.
+ * z / W in place between calls (re-weighting; robust factors of type 32 re-weight on the GPU at
+ * every linearisation instead), change a robust factor's loss, or swap a factor for another one.
  * The HBM mirror is checked against the host structs on every batch call: factors [0, upto) whose
  * measurement or information matrix changed are re-uploaded; a change of type or node ids is
  * reported through the return value (the symbolic plan has to be rebuilt).  The check costs one
@@ -287,9 +302,15 @@ static int gctx_verify_factors(gctx_t *c, april_graph_t *g, int upto)
             continue;
         }
         double *m = c->zw + 12 * (size_t) i;
-        if (memcmp(m, f->u.common.z, 3 * sizeof(double)) != 0 || memcmp(m + 3, Wm->data, 9 * sizeof(double)) != 0) {
+        int32_t loss;
+        double k;
+        asam_factor_loss(f, &loss, &k);
+        if (memcmp(m, f->u.common.z, 3 * sizeof(double)) != 0 || memcmp(m + 3, Wm->data, 9 * sizeof(double)) != 0 ||
+            loss != c->floss[i] || memcmp(&k, &c->fk[i], sizeof(double)) != 0) {
             memcpy(m, f->u.common.z, 3 * sizeof(double));
             memcpy(m + 3, Wm->data, 9 * sizeof(double));
+            c->floss[i] = loss;
+            c->fk[i] = k;
             changed = 1;
             if (i < lo)
                 lo = i;
@@ -305,11 +326,15 @@ static int gctx_verify_factors(gctx_t *c, april_graph_t *g, int upto)
     int cnt = hi - lo + 1;
     double *zw = malloc(sizeof(double) * 12 * (size_t) cnt);
     double *z = zw, *W = zw + 3 * (size_t) cnt;
+    int robust = 0;
     for (int k = 0; k < cnt; k++) {
         memcpy(z + 3 * (size_t) k, c->zw + 12 * (size_t) (lo + k), 3 * sizeof(double));
         memcpy(W + 9 * (size_t) k, c->zw + 12 * (size_t) (lo + k) + 3, 9 * sizeof(double));
+        robust |= c->floss[lo + k] != 0;
     }
     DEV_OK(asam_upload_factors(c->dev, lo, cnt, c->ftype + lo, c->fa + lo, c->fb + lo, z, W));
+    if (robust)
+        DEV_OK(asam_upload_loss(c->dev, lo, cnt, c->floss + lo, c->fk + lo));
     free(zw);
     return 1;
 }
@@ -991,7 +1016,7 @@ ASAM_API void april_graph_cholesky_inc(april_graph_t *graph, april_graph_cholesk
     tr->naffected = 0;
     for (int f = F0; f < F; f++) {
         int ends[2] = { c->fa[f], c->fb[f] };
-        for (int z0 = 0; z0 < (c->ftype[f] == APRIL_GRAPH_FACTOR_XYT_TYPE ? 2 : 1); z0++) {
+        for (int z0 = 0; z0 < (asam_two_pose_type(c->ftype[f]) ? 2 : 1); z0++) {
             search_tree_node_t *node = &tr->nodes[ends[z0]];
             while (!node->label_changed) {
                 node->label_changed = 1;
@@ -1005,12 +1030,12 @@ ASAM_API void april_graph_cholesky_inc(april_graph_t *graph, april_graph_cholesk
         }
     }
 
-    /* evaluation points of the new factors: l_point for xyt, state for xytpos */
+    /* evaluation points of the new factors: l_point for xyt (plain or robust), state for xytpos */
     int nf = F - F0;
     double *pts = gctx_stage(c, 6 * nf);
     for (int k = 0; k < nf; k++) {
         int f = F0 + k;
-        if (c->ftype[f] == APRIL_GRAPH_FACTOR_XYT_TYPE) {
+        if (asam_two_pose_type(c->ftype[f])) {
             memcpy(pts + 6 * (size_t) k, node_at(graph, c->fa[f])->l_point, 3 * sizeof(double));
             memcpy(pts + 6 * (size_t) k + 3, node_at(graph, c->fb[f])->l_point, 3 * sizeof(double));
         } else {

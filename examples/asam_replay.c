@@ -2,14 +2,18 @@
  *
  *   asam_replay --datapath FILE [--batch_update_only] [--delta_xy 0.1] [--delta_theta 0.1]
  *               [--nthreshold 100] [--quiet] [--show_timing] [--save OUT.graph]
+ *               [--robust huber:K | cauchy:K]
  *
  * FILE is a Manhattan-style text file (VERTEX2 id x y theta / EDGE2 a b dx dy dth I11 I12 I22 I33
  * I13 I23) or a ".graph" file in the stype framing.  The graph is then replayed pose by pose with
  * the protocol of the reference demo (examples/aprilsam_demo.c:150-234): step k appends pose k and
  * every factor whose larger pose id is k; the first step adds a prior on pose 0 and calls
  * april_graph_cholesky, every later step april_graph_cholesky_inc (or the batch call with
- * --batch_update_only); chi2 and the step time are printed per step.
- * Written against include/aprilsam/aprilsam.h only: it links unchanged against the reference too.
+ * --batch_update_only); chi2 and the step time are printed per step.  --robust creates every "scan" factor
+ * (a loop closure, |a - b| != 1) as a robust xyt factor with a Huber or Cauchy loss of scale K > 0, so that
+ * a wrong closure cannot pull the trajectory towards it.
+ * Written against include/aprilsam/aprilsam.h only: without --robust (an aprilsam_b200 extension) it links
+ * unchanged against the reference too.
  */
 #define _POSIX_C_SOURCE 200809L
 #include <math.h>
@@ -75,12 +79,40 @@ bad:
     return NULL;
 }
 
+/* "huber:K" or "cauchy:K" with a finite K > 0 -> loss code and K; -1 if malformed */
+static int parse_robust(const char *s, int *loss, double *k)
+{
+    const char *colon = strchr(s, ':');
+    if (!colon)
+        return -1;
+    size_t n = (size_t) (colon - s);
+    if (n == 5 && !strncmp(s, "huber", 5))
+        *loss = APRILSAM_B200_LOSS_HUBER;
+    else if (n == 6 && !strncmp(s, "cauchy", 6))
+        *loss = APRILSAM_B200_LOSS_CAUCHY;
+    else
+        return -1;
+    char *end;
+    *k = strtod(colon + 1, &end);
+    if (end == colon + 1 || *end || !(*k > 0.0) || !isfinite(*k))
+        return -1;
+    return 0;
+}
+
 int main(int argc, char **argv)
 {
     const char *path = NULL, *save = NULL;
-    int batch_only = 0, quiet = 0, nthreshold = 100, show_timing = 0;
-    double delta_xy = 0.1, delta_theta = 0.1;
+    int batch_only = 0, quiet = 0, nthreshold = 100, show_timing = 0, robust_loss = 0;
+    double delta_xy = 0.1, delta_theta = 0.1, robust_k = 0.0;
     for (int i = 1; i < argc; i++) {
+        if (!strcmp(argv[i], "--robust")) {
+            if (i + 1 >= argc || parse_robust(argv[i + 1], &robust_loss, &robust_k)) {
+                fprintf(stderr, "%s: --robust expects huber:K or cauchy:K with a finite K > 0\n", argv[0]);
+                return 2;
+            }
+            i++;
+            continue;
+        }
         if (!strcmp(argv[i], "--datapath") && i + 1 < argc) path = argv[++i];
         else if (!strcmp(argv[i], "--save") && i + 1 < argc) save = argv[++i];
         else if (!strcmp(argv[i], "--batch_update_only")) batch_only = 1;
@@ -91,7 +123,7 @@ int main(int argc, char **argv)
         else if (!strcmp(argv[i], "--nthreshold") && i + 1 < argc) nthreshold = atoi(argv[++i]);
         else {
             fprintf(stderr, "usage: %s --datapath FILE [--batch_update_only] [--delta_xy D] [--delta_theta D] "
-                            "[--nthreshold N] [--quiet] [--save OUT.graph]\n", argv[0]);
+                            "[--nthreshold N] [--quiet] [--save OUT.graph] [--robust huber:K | cauchy:K]\n", argv[0]);
             return 2;
         }
     }
@@ -158,8 +190,13 @@ int main(int argc, char **argv)
         for (int e = first[k]; e < first[k + 1]; e++) {
             april_graph_factor_t *fac;
             zarray_get(all->factors, order[e], &fac);
-            april_graph_factor_t *c = fac->copy(fac);
-            const char *type = april_graph_factor_attr_get(c, "type");
+            const char *type = april_graph_factor_attr_get(fac, "type");
+            april_graph_factor_t *c;
+            if (robust_loss && fac->type == APRIL_GRAPH_FACTOR_XYT_TYPE && type && !strcmp(type, "scan"))
+                c = aprilsam_b200_factor_xyt_robust_create(fac->nodes[0], fac->nodes[1], fac->u.common.z,
+                                                           fac->u.common.ztruth, fac->u.common.W, robust_loss, robust_k);
+            else
+                c = fac->copy(fac);
             if (c->nnodes == 2 && type && !strcmp(type, "odom")) {
                 /* dead-reckon the new pose from its neighbour and relinearise it */
                 int a = c->nodes[0], b = c->nodes[1];

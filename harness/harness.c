@@ -35,6 +35,9 @@ typedef struct hctx {
     double last_ms;
     /* replay cursor */
     int next_step;
+    /* loss / k of the robust factors h_replay and h_load_full create for "scan" edges (0: plain xyt) */
+    int scan_loss;
+    double scan_k;
 } hctx_t;
 
 static double now_ms(void)
@@ -101,6 +104,58 @@ H_EXPORT int h_add_xyt(hctx_t *h, int a, int b, const double *z, const double *W
     zarray_add(h->g->factors, &f);
     matd_destroy(W);
     return zarray_size(h->g->factors) - 1;
+}
+
+/* a robust xyt factor (aprilsam_b200 extension); -1 and no factor in the reference build or for invalid loss / k */
+H_EXPORT int h_add_xyt_robust(hctx_t *h, int a, int b, const double *z, const double *W9, int loss, double k)
+{
+#ifndef HARNESS_REFERENCE
+    matd_t *W = matd_create_data(3, 3, W9);
+    april_graph_factor_t *f = aprilsam_b200_factor_xyt_robust_create(a, b, z, NULL, W, loss, k);
+    matd_destroy(W);
+    if (!f)
+        return -1;
+    zarray_add(h->g->factors, &f);
+    return zarray_size(h->g->factors) - 1;
+#else
+    (void) h, (void) a, (void) b, (void) z, (void) W9, (void) loss, (void) k;
+    return -1;
+#endif
+}
+
+/* aprilsam_b200_factor_set_loss on factor idx: 0 ok, -1 otherwise (always -1 in the reference build) */
+H_EXPORT int h_set_loss(hctx_t *h, int idx, int loss, double k)
+{
+#ifndef HARNESS_REFERENCE
+    april_graph_factor_t *f;
+    zarray_get(h->g->factors, idx, &f);
+    return aprilsam_b200_factor_set_loss(f, loss, k);
+#else
+    (void) h, (void) idx, (void) loss, (void) k;
+    return -1;
+#endif
+}
+
+/* from now on h_replay / h_load_full create every "scan" edge (|a-b| != 1) as a robust factor with this loss;
+ * loss 0 = plain xyt (the default).  No-op in the reference build. */
+H_EXPORT void h_set_scan_loss(hctx_t *h, int loss, double k)
+{
+    h->scan_loss = loss;
+    h->scan_k = k;
+}
+
+static void add_edge(hctx_t *h, int a, int b, const double *z, const double *W9)
+{
+#ifndef HARNESS_REFERENCE
+    if (h->scan_loss && abs(a - b) != 1) {
+        if (h_add_xyt_robust(h, a, b, z, W9, h->scan_loss, h->scan_k) < 0) {
+            fprintf(stderr, "harness: %s\n", aprilsam_b200_last_error());
+            abort();
+        }
+        return;
+    }
+#endif
+    h_add_xyt(h, a, b, z, W9);
 }
 
 H_EXPORT int h_add_xytpos(hctx_t *h, int a, const double *z, const double *W9)
@@ -257,7 +312,7 @@ H_EXPORT int h_replay(hctx_t *h, int N, const double *init, const int *estart, c
                     na->relinearize(na);
                 }
             }
-            h_add_xyt(h, a, b, &ez[3 * e], &eW[9 * e]);
+            add_edge(h, a, b, &ez[3 * e], &eW[9 * e]);
         }
         double ms;
         if (k == 0 || batch_only)
@@ -286,7 +341,7 @@ H_EXPORT void h_load_full(hctx_t *h, int N, const double *init, int E, const int
     double z[3] = { 0, 0, 0 };
     h_add_xytpos(h, 0, z, W);
     for (int e = 0; e < E; e++)
-        h_add_xyt(h, ea[e], eb[e], &ez[3 * e], &eW[9 * e]);
+        add_edge(h, ea[e], eb[e], &ez[3 * e], &eW[9 * e]);
     h->next_step = N;
 }
 
@@ -386,6 +441,40 @@ H_EXPORT int h_factor(hctx_t *h, int idx, double *out)
     memcpy(out + 5, f->u.common.W->data, 9 * sizeof(double));
     return f->type;
 }
+
+/* the factor's host hook: which 0 = eval (at l_point), 1 = state_eval (at state).  out = r[3] | J_0[9] | J_1[9] |
+ * W[9] | chi2 (J_1 zero for unary factors); returns the residual length, -1 if the hook is not set */
+H_EXPORT int h_eval(hctx_t *h, int idx, int which, double *out)
+{
+    april_graph_factor_t *f;
+    zarray_get(h->g->factors, idx, &f);
+    april_graph_factor_eval_t *(*fn)(april_graph_factor_t *, april_graph_t *, april_graph_factor_eval_t *) =
+        which ? f->state_eval : f->eval;
+    if (!fn)
+        return -1;
+    april_graph_factor_eval_t *ev = fn(f, h->g, NULL);
+    memset(out, 0, 31 * sizeof(double));
+    memcpy(out, ev->r, 3 * sizeof(double));
+    for (int j = 0; j < 2 && ev->jacobians[j]; j++)
+        memcpy(out + 3 + 9 * j, ev->jacobians[j]->data, 9 * sizeof(double));
+    memcpy(out + 21, ev->W->data, 9 * sizeof(double));
+    out[30] = ev->chi2;
+    int len = ev->length;
+    april_graph_factor_eval_destroy(ev);
+    return len;
+}
+
+/* append factor->copy(factor) of factor idx; returns the new index */
+H_EXPORT int h_copy_factor(hctx_t *h, int idx)
+{
+    april_graph_factor_t *f;
+    zarray_get(h->g->factors, idx, &f);
+    april_graph_factor_t *c = f->copy(f);
+    zarray_add(h->g->factors, &c);
+    return zarray_size(h->g->factors) - 1;
+}
+
+H_EXPORT int h_dof(hctx_t *h) { return april_graph_dof(h->g); }
 
 /* overwrite measurement and information matrix of factor idx IN PLACE (what a robust-kernel or
  * re-weighting loop around the reference does between batch calls) */

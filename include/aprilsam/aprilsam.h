@@ -245,6 +245,23 @@ const char *aprilsam_b200_last_error(void);
  * values are re-checked on every batch call) -- it exists so that the uncached cost can be measured. */
 void aprilsam_b200_invalidate_plan(april_graph_cholesky_param_t *param);
 
+/* ---- robust loop closures (extension) ----------------------------------------------------------
+ * A type-32 factor is an xyt factor between two poses (same z, W, Jacobians and residual as type 1)
+ * with an M-estimator loss of scale k > 0.  At s = r'Wr (r at the factor's evaluation point):
+ *   Huber   w = 1 if s <= k^2, else k / sqrt(s)     rho = s if s <= k^2, else 2 k sqrt(s) - k^2
+ *   Cauchy  w = 1 / (1 + s / k^2)                   rho = k^2 log1p(s / k^2)
+ * Every linearisation uses W_eff = w W (iteratively reweighted least squares, no second-order term);
+ * april_graph_chi2 counts 0.5 rho(s) at the states.  The eval / state_eval hooks return W_eff and
+ * chi2 = rho(s).  Files holding such factors ("april_graph_factor_xyt_robust") are this library's own. */
+#define APRIL_GRAPH_FACTOR_XYT_ROBUST_TYPE 32
+enum { APRILSAM_B200_LOSS_HUBER = 1, APRILSAM_B200_LOSS_CAUCHY = 2 };
+/* NULL (text in aprilsam_b200_last_error) unless loss is one of the above and k is finite and > 0 */
+april_graph_factor_t *aprilsam_b200_factor_xyt_robust_create(int a, int b, const double *z, const double *ztruth,
+                                                             const matd_t *W, int loss, double k);
+/* change loss / k of a robust factor: 0 ok, -1 (and last_error) for another factor type or invalid values.
+ * Like an edit of z / W: used from the next batch solve on, not by incremental steps before it. */
+int aprilsam_b200_factor_set_loss(april_graph_factor_t *f, int loss, double k);
+
 /* Relinearisation / re-ordering policy of april_graph_cholesky_inc().  The reference escalates an
  * incremental step to a full batch solve when `start_over > nthreshold` (kept) and, as shipped, also
  * when the step took longer than a third of the last batch solve by the WALL CLOCK

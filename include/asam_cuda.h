@@ -62,6 +62,9 @@ int asam_reserve(asam_dev_t *d, int n_nodes, int n_factors, int n_slots, int n_s
 /* Graph mirror.  Factors are append-only (reference API has no removal). */
 int asam_upload_factors(asam_dev_t *d, int first, int count, const int32_t *type, const int32_t *na,
                         const int32_t *nb, const double *z3, const double *W9);
+/* Losses of robust xyt factors (type 32): per factor one 16-byte record {loss code as a double, k}
+ * (1 Huber, 2 Cauchy).  Only lanes of type-32 factors read it, so other factors may leave theirs unset. */
+int asam_upload_loss(asam_dev_t *d, int first, int count, const int32_t *loss, const double *k);
 /* which: 0 = l_point, 1 = state */
 int asam_upload_points(asam_dev_t *d, int which, int first, int count, const double *p3);
 /* copy poses [first, first+count) between the two mirrors inside HBM (which: 0 = l_point, 1 = state) */
@@ -168,7 +171,7 @@ int asam_download_y(asam_dev_t *d, int q_first, int q_count, double *y3);
 /* x and the factorisation status (see asam_factor_status) with a single synchronisation. */
 int asam_download_x_status(asam_dev_t *d, int q_first, int q_count, double *x3, int *status_out);
 
-/* chi2 = sum 0.5 r'Wr (xyt, at state) + sum r'Wr (xytpos) over factors [0, n_factors)
+/* chi2 = sum 0.5 r'Wr (xyt, at state) + sum 0.5 rho(r'Wr) (robust xyt) + sum r'Wr (xytpos) over factors [0, n_factors)
  * using the st mirror (april_graph.c:79-98). Deterministic reduction. */
 int asam_chi2(asam_dev_t *d, int n_factors, double *chi2_out);
 
@@ -185,10 +188,10 @@ int asam_factor_status(asam_dev_t *d, int *status_out);
 int asam_debug_read_hessian(asam_dev_t *d, int n_nodes, int n_slots, double *Adiag9, double *Aoff9, double *Bq3);
 int asam_debug_read_front(asam_dev_t *d, int64_t f_off, int64_t count, double *out);
 /* bytes [off, off+bytes) of one device mirror of host state: the plan (descriptors, int pool, node2q,
- * q2node, factor slots) or the factor mirror (type, node ids, z, W) */
+ * q2node, factor slots) or the factor mirror (type, node ids, z, W, {loss, k} records) */
 enum {
     ASAM_DBG_BUF_SN = 0, ASAM_DBG_BUF_IPOOL, ASAM_DBG_BUF_NODE2Q, ASAM_DBG_BUF_Q2NODE, ASAM_DBG_BUF_FSLOT,
-    ASAM_DBG_BUF_FTYPE, ASAM_DBG_BUF_FA, ASAM_DBG_BUF_FB, ASAM_DBG_BUF_FZ, ASAM_DBG_BUF_FW
+    ASAM_DBG_BUF_FTYPE, ASAM_DBG_BUF_FA, ASAM_DBG_BUF_FB, ASAM_DBG_BUF_FZ, ASAM_DBG_BUF_FW, ASAM_DBG_BUF_FLOSS
 };
 int asam_debug_read_buffer(asam_dev_t *d, int id, int64_t off, int64_t bytes, void *out);
 int asam_sync(asam_dev_t *d);

@@ -24,7 +24,12 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--poses", type=int, default=30000)
     ap.add_argument("--iters", type=int, default=5)
+    ap.add_argument("--robust", default=None, help="huber:K or cauchy:K: every loop closure a robust factor")
     args = ap.parse_args()
+    loss, k = 0, 0.0
+    if args.robust:
+        name, k = args.robust.split(":")
+        loss, k = {"huber": H.Harness.HUBER, "cauchy": H.Harness.CAUCHY}[name], float(k)
     import torch
     import torch.distributed as dist
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -38,6 +43,7 @@ def main():
     def run(shard: bool):
         capi.check(L.asam_comm_set_sharding(1 if shard else 0), "set_sharding")
         with H.Harness("b200") as h:
+            h.set_scan_loss(loss, k)
             h.load_full(d)
             h.batch()  # cold: plan
             dev = L.asam_dbg_dev_of_graph(h.graph_ptr())
