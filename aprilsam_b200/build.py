@@ -84,13 +84,13 @@ def build(force: bool = False, verbose: bool = False) -> str:
     hsrc = os.path.join(ROOT, "harness", "harness.c")
     if force or _stale(HARNESS, [hsrc, LIB] + hdrs):
         _run([CC, "-std=gnu99", "-O2", "-g", "-fPIC", "-shared", "-I" + os.path.join(ROOT, "include", "aprilsam"),
-              "-o", HARNESS, hsrc, "-L" + LIB_DIR, "-laprilsam_b200", "-Wl,-rpath," + LIB_DIR,
-              "-Wl,-rpath,$ORIGIN/../../aprilsam_b200/lib", "-lm"], log)
+              "-o", HARNESS, hsrc, "-L" + LIB_DIR, "-laprilsam_b200", "-Wl,-rpath,$ORIGIN/../../aprilsam_b200/lib", "-lm"],
+             log)
     csrc = os.path.join(ROOT, "examples", "asam_replay.c")
     os.makedirs(os.path.dirname(REPLAY_CLI), exist_ok=True)
     if force or _stale(REPLAY_CLI, [csrc, LIB] + hdrs):
         _run([CC, "-std=gnu99", "-O2", "-g", "-I" + os.path.join(ROOT, "include", "aprilsam"), "-o", REPLAY_CLI, csrc,
-              "-L" + LIB_DIR, "-laprilsam_b200", "-Wl,-rpath," + LIB_DIR, "-Wl,-rpath,$ORIGIN/../../aprilsam_b200/lib",
+              "-L" + LIB_DIR, "-laprilsam_b200", "-Wl,-rpath,$ORIGIN/../../aprilsam_b200/lib",
               "-lm"], log)
     # the oracle: C restatement always; the real reference, and its example programs linked against this
     # library, only where its sources exist

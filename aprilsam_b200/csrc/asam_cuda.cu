@@ -120,8 +120,6 @@ struct asam_dev {
     struct Pending *pend = nullptr;
     int npend = 0;
     int step_seq = 0;  // sequence number of the last k_step launch (completion flag in pin_down)
-    int tile_mode = 3; // ASAM_TILE_MODE (team path tiles): 0 DFMA, 1 mma.sync f64, 2 + bulk async copy per panel column,
-                       // 3 mma.sync f64, operands by rows from the panel workspace (two bulk copies per tile), fused crew items
     int pb_smem = 12;  // ASAM_PB_SMEM: panel width of shared-memory fronts
     int smem_mma = 1;  // ASAM_SMEM_MMA: 0 DFMA only, 1 tensor pipe for the kept-columns update, 2 for every panel update
     int solo_pb = 48;  // ASAM_SOLO_PB: staged panel width of single-CTA fronts that live in HBM
@@ -598,10 +596,6 @@ ASAM_EXPORT int asam_dev_create(asam_dev_t **out)
         d->pb_smem = atoi(getenv("ASAM_PB_SMEM")) / 3 * 3;
     if (getenv("ASAM_SMEM_MMA"))
         d->smem_mma = atoi(getenv("ASAM_SMEM_MMA"));
-    if (getenv("ASAM_DIAG_MMA")) {
-        const int v = atoi(getenv("ASAM_DIAG_MMA")) != 0;
-        CK(cudaMemcpyToSymbol(g_diag_mma, &v, sizeof(int)));
-    }
     if (getenv("ASAM_DMAP_AHEAD")) {
         const int v = atoi(getenv("ASAM_DMAP_AHEAD")) != 0;
         CK(cudaMemcpyToSymbol(g_dmap_ahead, &v, sizeof(int)));
@@ -612,8 +606,6 @@ ASAM_EXPORT int asam_dev_create(asam_dev_t **out)
     }
     if (getenv("ASAM_KEEP"))
         d->keep_off = atoi(getenv("ASAM_KEEP")) == 0;
-    if (getenv("ASAM_TILE_MODE"))
-        d->tile_mode = atoi(getenv("ASAM_TILE_MODE"));
     if (getenv("ASAM_SMALL_STEP"))
         d->small_ok = atoi(getenv("ASAM_SMALL_STEP")) != 0;
     memset(d->pin_down, 0, 64);
@@ -905,7 +897,6 @@ static int launch_factor(asam_dev *d, int ntasks, const int *tasks_dev, const in
     a.smem_doubles = d->fac_smem / (int) sizeof(double);
     a.spin_limit = ASAM_SPIN_LIMIT_NS;
     a.solo_pb = d->solo_pb;
-    a.tile_mode = d->tile_mode;
     a.smem_mma = d->smem_mma;
     a.pb_smem = d->pb_smem;
     a.trace = nullptr;

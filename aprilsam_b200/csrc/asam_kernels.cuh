@@ -402,7 +402,6 @@ struct FacArgs {
     int pb_smem;   // panel width of shared-memory fronts (multiple of 3)
     int smem_mma;  // shared-memory fronts on the FP64 tensor pipe: 1 = the one wide update of kept columns (incremental
                    // steps), 2 = also the 12-column panel updates, 0 = DFMA only
-    int tile_mode; // trailing-update tiles of the team path: 0 DFMA, 1 mma.sync f64, 2 mma.sync f64 + bulk async copies
     int solo_pb; // widest staged panel of a front that one CTA handles out of HBM (multiple of ASAM_PB)
     unsigned long long *ptrace; // optional: panel-step stamps of supernode ptrace_sn, [panel][worker < 8][8]
     int ptrace_sn, ptrace_panels;
@@ -534,7 +533,6 @@ __device__ __forceinline__ void bar_sub(const int nthreads) { asm volatile("bar.
 // dependent chain of every 3x3 step)
 __constant__ int g_pf_groups = 1; // ASAM_PF_GROUPS=0: one thread per row in the in-panel update of panel_factor (A/B)
 __constant__ int g_dmap_ahead = 1; // ASAM_DMAP_AHEAD=0: destination maps child by child inside the extend-add loop (A/B)
-__constant__ int g_diag_mma = 1;  // ASAM_DIAG_MMA=0: DFMA update inside the 48 x 48 diagonal block of the team path (A/B)
 
 __device__ __forceinline__ void panel_factor(double *P, int ldp, int k0, int pb, int m, int sn_id, int *err,
                                              double *dinv_out, const int sub_nt = 0)
@@ -622,12 +620,13 @@ __device__ __forceinline__ void panel_factor(double *P, int ldp, int k0, int pb,
 // Big fronts: a TEAM of G CTAs (consecutive tickets of the same supernode) factors one front that
 // does not fit in shared memory.  The front stays in HBM/L2; phases are separated by a team
 // barrier on a per-supernode counter (tbar; the last worker to leave a front zeroes it again):
-//   every worker: wait for the children, zero + assemble + extend-add its OWN columns
-//   -> [barrier] -> per panel of <= ASAM_TPB columns: { every worker factors the diagonal block
-//   redundantly in shared memory (left-looking 3-column steps), solves its 256-row chunks of the
-//   panel against it (rows in registers, 12 columns at a time) } -> [barrier] -> { tiles of the
-//   trailing update, L operands staged in shared memory, round-robin over workers } -> [barrier]
-// Column / chunk / tile ownership is a fixed function of (worker, team size): deterministic.
+//   every worker: wait for the children, zero + assemble + extend-add its OWN columns -> [barrier]
+//   -> panel 0 by everybody -> [barrier] -> per panel k of <= ASAM_TPB columns: { a crew factors panel
+//   k+1: worker 0 factors its diagonal block and publishes L11 in 12-column stages behind a release flag,
+//   the other crew workers solve their row chunks stage by stage; the rest of the team applies panel k
+//   to the trailing matrix in tiles, operands from the row-major panel workspace } -> [barrier]
+// (DESIGN §4 has the details.)  Column / chunk / tile ownership is a fixed function of (worker, team
+// size): deterministic.
 // All reads of front data written by other workers bypass L1 (ld.global.cg).
 // A supernode of this kind may be arbitrarily wide (host: fundamental chains of team-sized
 // fronts are merged without a cap), e.g. the 1383-column root separator of the 100 k graph.
@@ -637,13 +636,6 @@ __device__ __forceinline__ void panel_factor(double *P, int ldp, int k0, int pb,
 #define ASAM_TCOLS 64
 
 #define ASAM_CROWS 128 // rows of one look-ahead crew item (row chunk of the next panel)
-// Staged operands of the tensor-pipe tile: column p of the row operand at Li[p * ASAM_LDI], of the
-// column operand at Lj[p * ASAM_LDJ].  Both leading dimensions are = 4 (mod 16) doubles, which makes the
-// m8n8k4 fragment loads (8 consecutive rows x 4 consecutive panel columns per warp) bank-conflict free,
-// and even, so every staged column starts 16-byte aligned (bulk asynchronous copies).
-#define ASAM_LDI (ASAM_TROWS + 4)
-#define ASAM_LDJ (ASAM_TCOLS + 4)
-#define ASAM_TEAM_SMEM_DOUBLES (ASAM_TPB * ASAM_TPB + ASAM_TPB + ASAM_LDI * ASAM_TPB + ASAM_LDJ * ASAM_TPB)
 
 // ---- mbarrier / bulk asynchronous copy (TMA engine, 1-D) --------------------------------------------
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned) __cvta_generic_to_shared(p); }
@@ -682,132 +674,7 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, unsigned by
                  : "memory");
 }
 
-// C[rb0.., cb0..] -= L[rb0.., k0..k0+pb) * L[cb0.., k0..k0+pb)'  (lower trapezoid of the front only) on the
-// FP64 tensor pipe: mma.sync.m8n8k4.f64.  The operands are staged in shared memory (Li: nrow x pb, Lj: ncol x pb,
-// columns pb..pb4 zero) either by the threads (bulk == 0) or by the TMA engine: one bulk asynchronous copy
-// per panel column, completion on an mbarrier (bulk == 1; sources are rounded down to an even front row, the
-// fragment loads skip the extra leading row: shi / shj).  Warp w owns the 8*MT-row strip w of the tile and all
-// of its (at most 8) 8-column blocks: MT*8 accumulator fragments; per 4 panel columns MT + 8 shared-memory
-// fragment loads feed MT*8 tensor instructions of 256 multiply-adds each (the DFMA formulation needed 12 loads
-// per 1024 multiply-adds).  The C values are fetched before the products and written after them.
-// Dout != nullptr: the tile is the diagonal block of the next panel; its values also go straight into the
-// shared-memory block that diag_factor works on.
-template <int MT>
-__device__ __noinline__ void tile_mma(double *F, const int ld, const int m, const int k0, const int pb, const int cb0,
-                                         const int ncol, const int rb0, const int nrow, double *Dout, double *Li, double *Lj,
-                                         unsigned long long *bar, unsigned &parity, const int bulk)
-{
-    const int tid = threadIdx.x, nt = blockDim.x;
-    const int lane = tid & 31, warp = tid >> 5, nwarps = nt >> 5;
-    const int pb4 = (pb + 3) & ~3;
-    const int shi = bulk ? (rb0 & 1) : 0, shj = bulk ? (cb0 & 1) : 0;
-    __syncthreads(); // everybody is done with the previous contents of Li / Lj
-    if (bulk) {
-        const unsigned bi = (unsigned) ((shi + nrow + 1) & ~1) * 8u, bj = (unsigned) ((shj + ncol + 1) & ~1) * 8u;
-        if (warp == 0) {
-            asm volatile("fence.proxy.async;" ::: "memory"); // generic-proxy accesses (ours to shared memory, the other
-                                                             // workers' to the front) before the async-proxy copies
-            if (lane == 0)
-                mbar_expect_tx(bar, (unsigned) pb * (bi + bj));
-            __syncwarp();
-            for (int p = lane; p < pb; p += 32) {
-                const double *col = F + (size_t) (k0 + p) * ld;
-                bulk_g2s(Li + (size_t) p * ASAM_LDI, col + (rb0 - shi), bi, bar);
-                bulk_g2s(Lj + (size_t) p * ASAM_LDJ, col + (cb0 - shj), bj, bar);
-            }
-        }
-        for (int e = tid; e < (pb4 - pb) * ASAM_LDI; e += nt) // zero padding of the k dimension (last panel only)
-            Li[(size_t) pb * ASAM_LDI + e] = 0.0;
-        for (int e = tid; e < (pb4 - pb) * ASAM_LDJ; e += nt)
-            Lj[(size_t) pb * ASAM_LDJ + e] = 0.0;
-    } else {
-        // two panel columns per warp and pass: 20 independent loads in flight per lane
-        for (int p = warp; p < pb4; p += 2 * nwarps) {
-            double vj[2][2], vi[2][8];
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const int pp = p + h * nwarps;
-                const double *src = F + (size_t) (k0 + min(pp, pb - 1)) * ld;
-#pragma unroll
-                for (int u = 0; u < 2; u++)
-                    vj[h][u] = (pp < pb && lane + 32 * u < ncol) ? __ldcg(src + cb0 + lane + 32 * u) : 0.0;
-#pragma unroll
-                for (int u = 0; u < 8; u++)
-                    vi[h][u] = (pp < pb && lane + 32 * u < nrow) ? __ldcg(src + rb0 + lane + 32 * u) : 0.0;
-            }
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const int pp = p + h * nwarps;
-                if (pp < pb4) {
-#pragma unroll
-                    for (int u = 0; u < 2; u++)
-                        Lj[lane + 32 * u + pp * ASAM_LDJ] = vj[h][u];
-#pragma unroll
-                    for (int u = 0; u < 8; u++)
-                        Li[lane + 32 * u + pp * ASAM_LDI] = vi[h][u];
-                }
-            }
-        }
-    }
-    // this warp's strip and its accumulators, initialised with the C values
-    const int g = lane >> 2, t = lane & 3;
-    const int r0 = warp * 8 * MT;
-    const int nnt = (ncol + 7) >> 3;
-    // 8-column blocks that reach the strip's last row (lower trapezoid): nothing to do above the diagonal
-    const int rowmax = rb0 + min(r0 + 8 * MT, nrow) - 1;
-    const int nneed = (r0 < nrow && rowmax >= cb0) ? min(nnt, ((rowmax - cb0) >> 3) + 1) : 0;
-    double acc[MT][8][2];
-#pragma unroll
-    for (int mt = 0; mt < MT; mt++)
-#pragma unroll
-        for (int q = 0; q < 8; q++)
-#pragma unroll
-            for (int e = 0; e < 2; e++) {
-                const int ii = r0 + 8 * mt + g, jj = 8 * q + 2 * t + e;
-                const bool ok = q < nneed && ii < nrow && jj < ncol && rb0 + ii >= cb0 + jj;
-                acc[mt][q][e] = ok ? __ldcg(&F[(rb0 + ii) + (size_t) (cb0 + jj) * ld]) : 0.0;
-            }
-    if (bulk) {
-        mbar_wait(bar, parity);
-        parity ^= 1u;
-    }
-    __syncthreads(); // staged operands (and the zero padding) visible to every warp
-    if (nneed > 0) {
-        const double *ai = Li + shi + r0 + g + (size_t) t * ASAM_LDI;
-        const double *bj_ = Lj + shj + g + (size_t) t * ASAM_LDJ;
-#pragma unroll 2
-        for (int kk = 0; kk < pb4; kk += 4) {
-            double av[MT];
-#pragma unroll
-            for (int mt = 0; mt < MT; mt++)
-                av[mt] = -ai[8 * mt + (size_t) kk * ASAM_LDI];
-#pragma unroll
-            for (int q = 0; q < 8; q++) {
-                if (q < nneed) {
-                    const double bv = bj_[8 * q + (size_t) kk * ASAM_LDJ];
-#pragma unroll
-                    for (int mt = 0; mt < MT; mt++)
-                        dmma_8x8x4(acc[mt][q][0], acc[mt][q][1], av[mt], bv);
-                }
-            }
-        }
-#pragma unroll
-        for (int mt = 0; mt < MT; mt++)
-#pragma unroll
-            for (int q = 0; q < 8; q++)
-#pragma unroll
-                for (int e = 0; e < 2; e++) {
-                    const int ii = r0 + 8 * mt + g, jj = 8 * q + 2 * t + e;
-                    if (q < nneed && ii < nrow && jj < ncol && rb0 + ii >= cb0 + jj) {
-                        F[(rb0 + ii) + (size_t) (cb0 + jj) * ld] = acc[mt][q][e];
-                        if (Dout)
-                            Dout[ii + jj * ASAM_TPB] = acc[mt][q][e];
-                    }
-                }
-    }
-}
-
-// Row-major PANEL WORKSPACE of a team front (tile mode 3).  Behind the front (arena[f_off + ld*m ...]) sit two
+// Row-major PANEL WORKSPACE of a team front.  Behind the front (arena[f_off + ld*m ...]) sit two
 // buffers of (m+2) rows x ASAM_LDW doubles; buffer k&1 holds the factored panel k by ROWS: row r of the front
 // at W[r * ASAM_LDW .. + pb), zero up to the next multiple of 4.  A tile's operands -- a chunk of rows of the
 // panel -- are then ONE contiguous block each: two bulk asynchronous copies per tile instead of one per panel
@@ -818,9 +685,11 @@ __device__ __noinline__ void tile_mma(double *F, const int ld, const int m, cons
 
 // C[rb0.., cb0..] -= L[rb0.., panel] * L[cb0.., panel]' with the panel taken from its row-major workspace Wk.
 // out_mode 0: C is read from and written back to the front (trailing update); 1: C is read from the front and
-// written to Out[ii + jj * ASAM_TPB] (the next panel's diagonal block, for diag_factor); 2: C is read from the
-// front and written to Out[ii + jj * ASAM_TROWS] (rows of the next panel, solved in place by trsm_row; Out may
-// alias Li).  Same warp layout as tile_mma.
+// written to Out[ii + jj * ASAM_TPB] (the next panel's diagonal block, factored in diag_publish); 2: C is read from
+// the front and written to Out[ii + jj * ASAM_TROWS] (rows of the next panel, solved in place by trsm_row_block; Out
+// may alias Li).  FP64 tensor pipe (mma.sync.m8n8k4.f64): warp w owns the 8*MT-row strip w of the tile and all of
+// its (at most 8) 8-column blocks; per 4 panel columns MT + 8 shared-memory fragment loads feed MT*8 tensor
+// instructions.  The C values are fetched before the products and written after them.
 template <int MT>
 __device__ __noinline__ void tile_rm(double *F, const int ld, const double *Wk, const int pb4, const int cb0, const int ncol,
                                      const int rb0, const int nrow, const int out_mode, double *Out, double *Li, double *Lj,
@@ -947,66 +816,10 @@ __device__ __forceinline__ void team_leave(TeamCtx &tc)
 
 __device__ __forceinline__ bool team_owns(int col, int w, int G) { return ((col >> 2) % G) == w; }
 
-// Cholesky of the pb x pb diagonal block held in shared memory (column-major, leading dimension
-// ASAM_TPB), by all threads of the CTA: left-looking over 3-column steps (one pose each) -- the
-// three columns first receive the contributions of the columns to their left (one thread per
-// entry, a dot product), then a closed-form 3x3 Cholesky (evaluated redundantly, three chained
-// reciprocal square roots) finishes them.  rdv[k] = 1 / L_kk.
-__device__ __forceinline__ void diag_factor(double *D, int pb, double *rdv, int sn_id, int *err)
-{
-    const int tid = threadIdx.x;
-    constexpr int LDD = ASAM_TPB;
-    for (int c0 = 0; c0 < pb; c0 += 3) {
-        if (c0 > 0 && tid < 3 * (pb - c0)) {
-            const int i = c0 + tid / 3, j = c0 + tid % 3;
-            if (i >= j) {
-                double acc0 = D[i + j * LDD], acc1 = 0.0;
-                int p = 0;
-                for (; p + 1 < c0; p += 2) {
-                    acc0 -= D[i + p * LDD] * D[j + p * LDD];
-                    acc1 -= D[i + (p + 1) * LDD] * D[j + (p + 1) * LDD];
-                }
-                if (p < c0)
-                    acc0 -= D[i + p * LDD] * D[j + p * LDD];
-                D[i + j * LDD] = acc0 + acc1;
-            }
-        }
-        __syncthreads();
-        double *p0 = D + c0 * LDD, *p1 = p0 + LDD, *p2 = p1 + LDD;
-        const double a00 = p0[c0], a10 = p0[c0 + 1], a20 = p0[c0 + 2];
-        const double a11 = p1[c0 + 1], a21 = p1[c0 + 2], a22 = p2[c0 + 2];
-        const double r0 = d_rsqrt(a00);
-        const double l10 = a10 * r0, l20 = a20 * r0;
-        const double d1 = a11 - l10 * l10;
-        const double r1 = d_rsqrt(d1);
-        const double l21 = (a21 - l20 * l10) * r1;
-        const double d2 = a22 - l20 * l20 - l21 * l21;
-        const double r2 = d_rsqrt(d2);
-        if (tid == 0 && !(a00 > 0.0 && d1 > 0.0 && d2 > 0.0))
-            atomicCAS(err, 0, 1 + sn_id);
-        const int i = c0 + 3 + tid;
-        if (i < pb) {
-            const double x0 = p0[i] * r0;
-            const double x1 = (p1[i] - x0 * l10) * r1;
-            const double x2 = (p2[i] - x0 * l20 - x1 * l21) * r2;
-            p0[i] = x0;
-            p1[i] = x1;
-            p2[i] = x2;
-        }
-        __syncthreads();
-        if (tid == 0) {
-            p0[c0] = a00 * r0; p0[c0 + 1] = l10; p0[c0 + 2] = l20;
-            p1[c0 + 1] = d1 * r1; p1[c0 + 2] = l21;
-            p2[c0 + 2] = d2 * r2;
-            rdv[c0] = r0; rdv[c0 + 1] = r1; rdv[c0 + 2] = r2;
-        }
-    }
-    __syncthreads();
-}
-
-// Same result, right-looking and blocked: 12-column sub-panels of closed-form 3x3 steps (panel_factor: every
-// thread of the CTA takes part in the row solves and the in-panel rank-3 updates) followed by a register-tiled
-// update of the rest of the block -- no dot products of growing length on the dependent chain.
+// Cholesky of the pb x pb diagonal block held in shared memory (column-major, leading dimension ASAM_TPB),
+// right-looking and blocked: 12-column sub-panels of closed-form 3x3 steps (panel_factor: every thread of the CTA
+// takes part in the row solves and the in-panel rank-3 updates) followed by an update of the rest of the block on
+// the FP64 tensor pipe -- no dot products of growing length on the dependent chain.  rdv[k] = 1 / L_kk.
 // Ends with a CTA-wide barrier.
 __device__ __forceinline__ void diag_factor_rl(double *D, int pb, double *rdv, int sn_id, int *err)
 {
@@ -1017,10 +830,7 @@ __device__ __forceinline__ void diag_factor_rl(double *D, int pb, double *rdv, i
             const int pbb = min(ASAM_PB, pb - k1);
             panel_factor(D + (size_t) k1 * LDD, LDD, k1, pbb, pb - 1, sn_id, err, rdv, SUB);
             if (k1 + pbb < pb) {
-                if (g_diag_mma)
-                    trailing_update_mma(D, LDD, D + (size_t) k1 * LDD, LDD, pbb, k1 + pbb, pb, pb - 1, SUB / 32);
-                else
-                    trailing_update<1, 4>(D, LDD, D + (size_t) k1 * LDD, LDD, pbb, k1 + pbb, pb, pb - 1, SUB / 32);
+                trailing_update_mma(D, LDD, D + (size_t) k1 * LDD, LDD, pbb, k1 + pbb, pb, pb - 1, SUB / 32);
                 bar_sub(SUB);
             }
         }
@@ -1031,9 +841,9 @@ __device__ __forceinline__ void diag_factor_rl(double *D, int pb, double *rdv, i
 // One row of the panel per thread: x = row * L11^-T.  The row lives in Li (column p at
 // Li[tid + p*ASAM_TROWS]); it is processed 12 columns at a time in registers -- first the
 // contributions of the columns already solved (L entries fetched two at a time, broadcast), then
-// the 12x12 triangle fully unrolled.  Results go back to Li and to the front in HBM.
-// Wrow != nullptr: the solved row also goes to the row-major panel workspace (Wrow[0..pb), zero up to the next
-// multiple of 4), where the next iteration's tiles fetch it as part of one contiguous block.
+// the 12x12 triangle fully unrolled.  Results go back to Li, to the front in HBM and to the row-major panel
+// workspace (Wrow[0..pb), zero up to the next multiple of 4), where the next iteration's tiles fetch it as part of
+// one contiguous block.
 // one 12-column block [b0, b0+nb) of the row solve (needs x of the columns before b0 in Li and rows b0.. of the
 // columns [0, b0+nb) of L11 in D)
 __device__ __forceinline__ void trsm_row_block(double *Li, const double *D, const double *rdv, const int b0, const int nb,
@@ -1069,19 +879,17 @@ __device__ __forceinline__ void trsm_row_block(double *Li, const double *D, cons
         if (q < nb) {
             Li[tid + (b0 + q) * ASAM_TROWS] = r[q];
             Frow[(size_t) (b0 + q) * ld] = r[q];
-            if (Wrow)
-                Wrow[b0 + q] = r[q];
+            Wrow[b0 + q] = r[q];
         }
 }
 
 __device__ __forceinline__ void trsm_row(double *Li, const double *D, const double *rdv, int pb, double *Frow, int ld,
-                                         double *Wrow = nullptr)
+                                         double *Wrow)
 {
     for (int b0 = 0; b0 < pb; b0 += 12)
         trsm_row_block(Li, D, rdv, b0, min(12, pb - b0), Frow, ld, Wrow);
-    if (Wrow)
-        for (int q = pb; q < ((pb + 3) & ~3); q++)
-            Wrow[q] = 0.0;
+    for (int q = pb; q < ((pb + 3) & ~3); q++)
+        Wrow[q] = 0.0;
 }
 
 // returns false on abort
@@ -1209,135 +1017,37 @@ __device__ bool team_front(const FacArgs &a, const asam_sn_desc_t &d, int s, int
     // ---- panels, with one panel of look-ahead ---------------------------------------------------
     // Panel k+1 is factored by a small CREW while the other workers are still applying panel k to
     // the rest of the trailing matrix.  In iteration k
-    //   crew worker 0:   applies panel k to the 48x48 diagonal block of panel k+1, factors it (once,
-    //                    left-looking 3-column steps), writes L11 / 1/diag and raises a flag
-    //   crew worker w>0: applies panel k to its 256-row chunk of panel k+1's columns (as long as the
-    //                    factorisation of the block takes), waits for the flag, solves its rows
+    //   crew worker 0:   applies panel k to the 48x48 diagonal block of panel k+1, factors it (once)
+    //                    and publishes L11 / 1/diag in 12-column stages, each behind a release flag
+    //   crew worker w>0: applies panel k to its 128-row chunk of panel k+1's columns, keeps the rows in
+    //                    shared memory and solves them stage by stage as the stages are published
     //   everybody else:  tiles of the trailing update with panel k right of panel k+1
     //   -> [team barrier]
     // so the dependent chain per panel is max(chunk update, block update + factorisation) + row solve
     // + one barrier, instead of factorisation + barrier + a whole trailing update + barrier.
     double *D = sm;                              // ASAM_TPB x ASAM_TPB diagonal block
     double *rdv = D + ASAM_TPB * ASAM_TPB;       // ASAM_TPB reciprocal diagonal entries
-    double *Li = rdv + ASAM_TPB;                 // ASAM_LDI x pb   (row chunk / row tile)
-    double *Lj = Li + ASAM_LDI * ASAM_TPB;       // ASAM_LDJ x pb   (column tile)
-    // tile mode 3: operands by rows from the panel workspace behind the front (Li: <= 256 x ASAM_LDW, Lj: <= 64 x ASAM_LDW)
-    const bool v3 = a.tile_mode == 3;
+    // tile operands by rows from the panel workspace behind the front (Li: <= 256 x ASAM_LDW, Lj: <= 64 x ASAM_LDW);
+    // Li also holds the rows being solved (column p at Li[tid + p * ASAM_TROWS])
+    double *Li = rdv + ASAM_TPB;
+    double *Lj = Li + ASAM_TROWS * ASAM_LDW;
     double *Wbase = F + (size_t) ld * m;
     auto Wbuf = [&](int panel_index) { return Wbase + (size_t) (panel_index & 1) * (m + 2) * ASAM_LDW; };
-    double *Lj3 = Li + ASAM_TROWS * ASAM_LDW;
     double *dinv = a.dinv + 3 * (size_t) d.first;
-    int *crew_bar = a.tbar + 2 * (size_t) s + 1; // flag: index (1-based) of the last published panel
+    int *crew_bar = a.tbar + 2 * (size_t) s + 1; // flag: 8 * seq + the stages of the diagonal block published
 
-    // C[rb0.., cb0..] -= L[rb0.., k0..k0+pb) * L[cb0.., k0..k0+pb)'  (lower trapezoid only)
-    // (Dout != nullptr: the tile is the diagonal block of the next panel; its values also go straight
-    // into the shared-memory block that diag_factor works on, saving the round trip through L2)
+    // C[rb0.., cb0..] -= L[rb0.., k0..k0+pb) * L[cb0.., k0..k0+pb)'  (lower trapezoid only), operands from the
+    // row-major workspace of the panel at k0.  Dout != nullptr: the tile is the diagonal block of the next panel;
+    // its values go straight into the shared-memory block that diag_publish factors, not back to the front
     auto tile = [&](int k0, int pb, int cb0, int ncol, int rb0, int nrow, double *Dout) {
-        if (v3) { // operands from the row-major workspace of the panel at k0; Dout: the next panel's diagonal block
-            const double *Wk = Wbuf(k0 / ASAM_TPB);
-            const int pb4 = (pb + 3) & ~3;
-            if (Dout)
-                tile_rm<1>(F, ld, Wk, pb4, cb0, ncol, rb0, nrow, 1, Dout, Li, Lj3, mbar, mb_parity);
-            else if (nrow <= 128)
-                tile_rm<2>(F, ld, Wk, pb4, cb0, ncol, rb0, nrow, 0, nullptr, Li, Lj3, mbar, mb_parity);
-            else
-                tile_rm<4>(F, ld, Wk, pb4, cb0, ncol, rb0, nrow, 0, nullptr, Li, Lj3, mbar, mb_parity);
-            return;
-        }
-        if (a.tile_mode != 0) { // FP64 tensor pipe (1: operands staged by the threads, 2: by bulk asynchronous copies)
-            const int bulk = a.tile_mode == 2;
-            if (nrow <= 64)
-                tile_mma<1>(F, ld, m, k0, pb, cb0, ncol, rb0, nrow, Dout, Li, Lj, mbar, mb_parity, bulk);
-            else if (nrow <= 128)
-                tile_mma<2>(F, ld, m, k0, pb, cb0, ncol, rb0, nrow, Dout, Li, Lj, mbar, mb_parity, bulk);
-            else
-                tile_mma<4>(F, ld, m, k0, pb, cb0, ncol, rb0, nrow, Dout, Li, Lj, mbar, mb_parity, bulk);
-            return;
-        }
-        // DFMA formulation (ASAM_TILE_MODE=0, kept for A/B measurements)
-        __syncthreads();
-        // two panel columns per warp and pass: 20 independent loads in flight per lane
-        for (int p = warp; p < pb; p += 2 * nwarps) {
-            double vj[2][2], vi[2][8];
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const int pp = p + h * nwarps;
-                const double *src = F + (size_t) (k0 + min(pp, pb - 1)) * ld;
-#pragma unroll
-                for (int u = 0; u < 2; u++)
-                    vj[h][u] = (pp < pb && lane + 32 * u < ncol) ? __ldcg(src + cb0 + lane + 32 * u) : 0.0;
-#pragma unroll
-                for (int u = 0; u < 8; u++)
-                    vi[h][u] = (pp < pb && lane + 32 * u < nrow) ? __ldcg(src + rb0 + lane + 32 * u) : 0.0;
-            }
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const int pp = p + h * nwarps;
-                if (pp < pb) {
-#pragma unroll
-                    for (int u = 0; u < 2; u++)
-                        if (lane + 32 * u < ncol)
-                            Lj[lane + 32 * u + pp * ASAM_TCOLS] = vj[h][u];
-#pragma unroll
-                    for (int u = 0; u < 8; u++)
-                        if (lane + 32 * u < nrow)
-                            Li[lane + 32 * u + pp * ASAM_TROWS] = vi[h][u];
-                }
-            }
-        }
-        __syncthreads();
-        // warp -> 8 columns, lane -> rows lane + 32 r (passes of 128 rows)
-        const int tj = 8 * warp;
-        if (tj < ncol) {
-            for (int ib = 0; ib < nrow; ib += 128) {
-                double acc[4][8], cv[4][8];
-                int ir[4], jc[8];
-#pragma unroll
-                for (int q = 0; q < 8; q++)
-                    jc[q] = min(tj + q, ncol - 1);
-#pragma unroll
-                for (int r = 0; r < 4; r++) {
-                    ir[r] = min(ib + lane + 32 * r, nrow - 1);
-#pragma unroll
-                    for (int q = 0; q < 8; q++) {
-                        acc[r][q] = 0.0;
-                        // the C values are fetched now and consumed after the products:
-                        // their L2 latency hides behind the 4x8xpb FMAs
-                        const int ii = ib + lane + 32 * r, jj = tj + q;
-                        const bool ok = ii < nrow && jj < ncol && rb0 + ii >= cb0 + jj;
-                        cv[r][q] = ok ? __ldcg(&F[(rb0 + ii) + (size_t) (cb0 + jj) * ld]) : 0.0;
-                    }
-                }
-#pragma unroll 2
-                for (int p = 0; p < pb; p++) {
-                    double bq[8], av[4];
-#pragma unroll
-                    for (int q = 0; q < 8; q++)
-                        bq[q] = Lj[jc[q] + p * ASAM_TCOLS];
-#pragma unroll
-                    for (int r = 0; r < 4; r++)
-                        av[r] = Li[ir[r] + p * ASAM_TROWS];
-#pragma unroll
-                    for (int r = 0; r < 4; r++)
-#pragma unroll
-                        for (int q = 0; q < 8; q++)
-                            acc[r][q] += av[r] * bq[q];
-                }
-#pragma unroll
-                for (int r = 0; r < 4; r++)
-#pragma unroll
-                    for (int q = 0; q < 8; q++) {
-                        const int ii = ib + lane + 32 * r, jj = tj + q;
-                        const int i = rb0 + ii, j = cb0 + jj;
-                        if (ii < nrow && jj < ncol && i >= j) {
-                            const double v = cv[r][q] - acc[r][q];
-                            F[i + (size_t) j * ld] = v;
-                            if (Dout)
-                                Dout[ii + jj * ASAM_TPB] = v;
-                        }
-                    }
-            }
-        }
+        const double *Wk = Wbuf(k0 / ASAM_TPB);
+        const int pb4 = (pb + 3) & ~3;
+        if (Dout)
+            tile_rm<1>(F, ld, Wk, pb4, cb0, ncol, rb0, nrow, 1, Dout, Li, Lj, mbar, mb_parity);
+        else if (nrow <= 128)
+            tile_rm<2>(F, ld, Wk, pb4, cb0, ncol, rb0, nrow, 0, nullptr, Li, Lj, mbar, mb_parity);
+        else
+            tile_rm<4>(F, ld, Wk, pb4, cb0, ncol, rb0, nrow, 0, nullptr, Li, Lj, mbar, mb_parity);
     };
     // diagonal block of the panel at k0 into D (every caller redundantly), the caller's row chunk
     // [rb0, rb0+256) below the block into Li while the block is being factored, then the rows
@@ -1353,12 +1063,9 @@ __device__ bool team_front(const FacArgs &a, const asam_sn_desc_t &d, int s, int
             for (int j = 0; j < pb; j++)
                 Li[tid + j * ASAM_TROWS] = __ldcg(&F[i + (size_t) (k0 + j) * ld]);
         __syncthreads();
-        if (v3)
-            diag_factor_rl(D, pb, rdv, s, err);
-        else
-            diag_factor(D, pb, rdv, s, err);
+        diag_factor_rl(D, pb, rdv, s, err);
         if (row)
-            trsm_row(Li, D, rdv, pb, F + i + (size_t) k0 * ld, ld, v3 ? Wbuf(0) + (size_t) i * ASAM_LDW : nullptr);
+            trsm_row(Li, D, rdv, pb, F + i + (size_t) k0 * ld, ld, Wbuf(0) + (size_t) i * ASAM_LDW);
     };
     auto writeback = [&](int k0, int pb) { // worker 0, after a team barrier: nobody reads the raw block any more
         for (int e = tid; e < pb * pb; e += nt) {
@@ -1370,54 +1077,40 @@ __device__ bool team_front(const FacArgs &a, const asam_sn_desc_t &d, int s, int
             dinv[k0 + e] = rdv[e];
     };
 
-    // worker 0 of the crew: the diagonal block of the panel at k0 (already updated by its own tile) is
-    // factored ONCE and published -- L11 into the front, 1/diag into dinv, then the flag
+    // worker 0 of the crew: the diagonal block of the panel at k0 (already updated by its own tile) is factored
+    // ONCE, blocked right-looking, and PUBLISHED IN STAGES: after each 12-column sub-panel its columns of L11 are
+    // final and go to the front + 1/diag to dinv + the flag (8 * seq + stage); the crew solves the matching 12
+    // columns of its rows while the next sub-panel is being factored, instead of starting when all 48 are done
     auto diag_publish = [&](int k0, int pb, int seq) {
         __syncthreads(); // D was zeroed before, and filled by, the tile that updated this block
-        if (v3) {
-            // blocked right-looking, PUBLISHED IN STAGES: after each 12-column sub-panel its columns of L11 are final
-            // and go to the front + the flag (8 * seq + stage); the crew solves the matching 12 columns of its rows
-            // while the next sub-panel is being factored, instead of starting when all 48 are done
-            constexpr int LDD = ASAM_TPB;
-            constexpr int SUB = 256; // threads that factor the block (one warp in registers, and 64 threads on a two-warp
-                                     // barrier, were SLOWER: the publish / update loops want the threads more than the
-                                     // barriers cost)
-            int stage = 0;
-            for (int k1 = 0; k1 < pb; k1 += ASAM_PB) {
-                const int pbb = min(ASAM_PB, pb - k1);
-                panel_factor(D + (size_t) k1 * LDD, LDD, k1, pbb, pb - 1, s, err, rdv, SUB);
-                ++stage;
-                for (int e = tid; e < pbb * pb; e += SUB) {
-                    const int j = k1 + e / pb, i = e % pb;
-                    if (i >= j)
-                        F[(k0 + i) + (size_t) (k0 + j) * ld] = D[i + j * LDD];
-                }
-                for (int e = tid; e < pbb; e += SUB)
-                    dinv[k0 + k1 + e] = rdv[k1 + e];
-                bar_sub(SUB);
-                if (tid == 0)
-                    st_release(crew_bar, 8 * seq + stage);
-                if (k1 + pbb < pb) {
-                    if (g_diag_mma)
-                        trailing_update_mma(D, LDD, D + (size_t) k1 * LDD, LDD, pbb, k1 + pbb, pb, pb - 1, SUB / 32);
-                    else
-                        trailing_update<1, 4>(D, LDD, D + (size_t) k1 * LDD, LDD, pbb, k1 + pbb, pb, pb - 1, SUB / 32);
-                    bar_sub(SUB);
-                }
+        constexpr int LDD = ASAM_TPB;
+        constexpr int SUB = 256; // threads that factor the block (one warp in registers, and 64 threads on a two-warp
+                                 // barrier, were SLOWER: the publish / update loops want the threads more than the
+                                 // barriers cost)
+        int stage = 0;
+        for (int k1 = 0; k1 < pb; k1 += ASAM_PB) {
+            const int pbb = min(ASAM_PB, pb - k1);
+            panel_factor(D + (size_t) k1 * LDD, LDD, k1, pbb, pb - 1, s, err, rdv, SUB);
+            ++stage;
+            for (int e = tid; e < pbb * pb; e += SUB) {
+                const int j = k1 + e / pb, i = e % pb;
+                if (i >= j)
+                    F[(k0 + i) + (size_t) (k0 + j) * ld] = D[i + j * LDD];
             }
-            __syncthreads();
-            return;
+            for (int e = tid; e < pbb; e += SUB)
+                dinv[k0 + k1 + e] = rdv[k1 + e];
+            bar_sub(SUB);
+            if (tid == 0)
+                st_release(crew_bar, 8 * seq + stage);
+            if (k1 + pbb < pb) {
+                trailing_update_mma(D, LDD, D + (size_t) k1 * LDD, LDD, pbb, k1 + pbb, pb, pb - 1, SUB / 32);
+                bar_sub(SUB);
+            }
         }
-        diag_factor(D, pb, rdv, s, err);
-        writeback(k0, pb);
         __syncthreads();
-        if (tid == 0) {
-            __threadfence();
-            atomicExch(crew_bar, seq);
-        }
     };
-    // tile mode 3: the crew's rows (already updated, in Li) are solved 12 columns at a time, each stage as soon as
-    // worker 0 has published the matching columns of L11
+    // the crew's rows (already updated, in Li) are solved 12 columns at a time, each stage as soon as worker 0 has
+    // published the matching columns of L11
     auto rows_solve_staged = [&](int k0, int pb, int rb0, int seq, double *Wnext) {
         constexpr int LDD = ASAM_TPB;
         // Two groups of four warps.  LOADERS (warps 4-7): wait for the flag of stage s, fetch its 12 columns of L11
@@ -1470,44 +1163,6 @@ __device__ bool team_front(const FacArgs &a, const asam_sn_desc_t &d, int s, int
         __syncthreads();
         return *s_flag != 0;
     };
-    // the other crew workers: rows [rb0, rb0+ASAM_CROWS) of the panel are fetched while worker 0 factors the
-    // block, then solved against the published L11
-    auto rows_solve = [&](int k0, int pb, int rb0, int seq, double *Wnext) {
-        __syncthreads();
-        const int i = rb0 + tid;
-        const bool row = tid < ASAM_CROWS && i <= m;
-        if (row && !Wnext) // (tile mode 3: the tile left the updated rows in Li already)
-            for (int j = 0; j < pb; j++)
-                Li[tid + j * ASAM_TROWS] = __ldcg(&F[i + (size_t) (k0 + j) * ld]);
-        if (tid == 0) {
-            SpinClock spins;
-            int ok = 1;
-            while (ld_volatile(crew_bar) < seq) {
-                __nanosleep(20);
-                if (spin_over(spins, a.spin_limit) || ld_volatile(err) < 0) {
-                    atomicCAS(err, 0, -(1 + s));
-                    ok = 0;
-                    break;
-                }
-            }
-            __threadfence();
-            *s_flag = ok;
-        }
-        __syncthreads();
-        if (!*s_flag)
-            return false;
-        for (int e = tid; e < ASAM_TPB * ASAM_TPB; e += nt) {
-            const int ii = e % ASAM_TPB, j = e / ASAM_TPB;
-            D[e] = (ii >= j && ii < pb && j < pb) ? __ldcg(&F[(k0 + ii) + (size_t) (k0 + j) * ld]) : 0.0;
-        }
-        for (int e = tid; e < ASAM_TPB; e += nt)
-            rdv[e] = e < pb ? __ldcg(&dinv[k0 + e]) : 0.0;
-        __syncthreads();
-        if (row)
-            trsm_row(Li, D, rdv, pb, F + i + (size_t) k0 * ld, ld, Wnext ? Wnext + (size_t) i * ASAM_LDW : nullptr);
-        return true;
-    };
-
     // prologue: panel 0 by everybody (row chunks of 256 from the panel's first row, round-robin)
     {
         const int pb = min(ASAM_TPB, c);
@@ -1561,31 +1216,17 @@ __device__ bool team_front(const FacArgs &a, const asam_sn_desc_t &d, int s, int
                 if (pt)
                     pt[2] = d_now();
             }
-            if (v3) {
-                // fused crew item: the updated rows go from the tensor-pipe accumulators straight into shared
-                // memory (no round trip through the front), are solved there against the published L11 and
-                // leave once -- to the front (final L) and to the next panel's row-major workspace
-                for (int it = (w == 0 ? G : w); it < ncrew; it += G) {
-                    const int rb0 = kn0 + pbn + (it - 1) * ASAM_CROWS;
-                    tile_rm<2>(F, ld, Wbuf(k0 / ASAM_TPB), (pb + 3) & ~3, kn0, pbn, rb0, min(ASAM_CROWS, m - rb0 + 1), 2, Li, Li,
-                               Lj3, mbar, mb_parity);
-                    if (pt && w > 0 && it == w)
-                        pt[1] = d_now();
-                    if (!rows_solve_staged(kn0, pbn, rb0, seq, Wbuf(kn0 / ASAM_TPB)))
-                        return false;
-                }
-            } else {
-                for (int it = (w == 0 ? G : w); it < ncrew; it += G) {
-                    const int rb0 = kn0 + pbn + (it - 1) * ASAM_CROWS;
-                    tile(k0, pb, kn0, pbn, rb0, min(ASAM_CROWS, m - rb0 + 1), nullptr);
-                }
-                if (pt && w > 0)
+            // fused crew item: the updated rows go from the tensor-pipe accumulators straight into shared
+            // memory (no round trip through the front), are solved there against the published L11 and
+            // leave once -- to the front (final L) and to the next panel's row-major workspace
+            for (int it = (w == 0 ? G : w); it < ncrew; it += G) {
+                const int rb0 = kn0 + pbn + (it - 1) * ASAM_CROWS;
+                tile_rm<2>(F, ld, Wbuf(k0 / ASAM_TPB), (pb + 3) & ~3, kn0, pbn, rb0, min(ASAM_CROWS, m - rb0 + 1), 2, Li, Li,
+                           Lj, mbar, mb_parity);
+                if (pt && w > 0 && it == w)
                     pt[1] = d_now();
-                for (int it = (w == 0 ? G : w); it < ncrew; it += G) {
-                    const int rb0 = kn0 + pbn + (it - 1) * ASAM_CROWS;
-                    if (!rows_solve(kn0, pbn, rb0, seq, nullptr))
-                        return false;
-                }
+                if (!rows_solve_staged(kn0, pbn, rb0, seq, Wbuf(kn0 / ASAM_TPB)))
+                    return false;
             }
             if (pt && w > 0)
                 pt[2] = d_now();

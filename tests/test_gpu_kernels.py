@@ -525,10 +525,11 @@ def test_pivots_outside_float_range(m3500, which):
 # ---------------------------------------------------------------------------------------------
 SWITCH_ZOO = ("smem159_c12", "smem_n51", "team162_c51", "team_chunk130", "bs_195", "wide")
 SWITCHES = {
-    "tile0": {"ASAM_TILE_MODE": "0"}, "tile1": {"ASAM_TILE_MODE": "1"}, "tile2": {"ASAM_TILE_MODE": "2"},
-    "diag_mma0": {"ASAM_DIAG_MMA": "0"}, "pf_groups0": {"ASAM_PF_GROUPS": "0"}, "dmap_ahead0": {"ASAM_DMAP_AHEAD": "0"},
+    "pf_groups0": {"ASAM_PF_GROUPS": "0"}, "dmap_ahead0": {"ASAM_DMAP_AHEAD": "0"},
     "smem_mma2": {"ASAM_SMEM_MMA": "2"}, "pb_smem24": {"ASAM_PB_SMEM": "24"},
-    "solo400": {"ASAM_SOLO_MAX_M": "400"}, "tpw2": {"ASAM_TILES_PER_WORKER": "2"},
+    "solo400": {"ASAM_SOLO_MAX_M": "400"}, "solo400_pb24": {"ASAM_SOLO_MAX_M": "400", "ASAM_SOLO_PB": "24"},
+    "solo400_pb12": {"ASAM_SOLO_MAX_M": "400", "ASAM_SOLO_PB": "12"}, "tpw2": {"ASAM_TILES_PER_WORKER": "2"},
+    "merge_pct0": {"ASAM_TEAM_MERGE_PCT": "0"}, "plan_threads1": {"ASAM_PLAN_THREADS": "1"},
     "bs_threads128": {"ASAM_BS_THREADS": "128"},
     "order_level": {"ASAM_TASK_ORDER": "level"}, "order_cp": {"ASAM_TASK_ORDER": "cp"},
     "order_sim": {"ASAM_TASK_ORDER": "sim"}, "bs_order_level": {"ASAM_BS_ORDER": "level"},

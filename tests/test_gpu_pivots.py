@@ -3,8 +3,8 @@ the double range, and a clean context after a failure.
 
 The status word (asam_factor_status, asam_download_x_status) is all that stands between an indefinite system and a
 wrong solution returned without complaint.  Each kernel path computes its own Cholesky pivots and flags a failure with
-its own atomicCAS(err, 0, 1 + s): panel_factor (cta_front in shared memory and out of HBM, the team diagonal block at
-tile mode 3), diag_factor (tile modes 0-2) and the warp loop of k_factor_leaf.
+its own atomicCAS(err, 0, 1 + s): panel_factor (cta_front in shared memory and out of HBM, the team diagonal block)
+and the warp loop of k_factor_leaf.
 
 How a failure is placed: the graph gets extra xytpos priors (SPD W; priors add no edges, so the plan is unchanged) on
 the poses to be targeted and is solved once through the public API.  After that only the C-ABI is used on its device
@@ -63,12 +63,11 @@ GROUPS = {
     "smem_mma2": ({"ASAM_SMEM_MMA": "2"}, _SMEM),
     "pb_smem24": ({"ASAM_PB_SMEM": "24"}, _SMEM),
     "cta_hbm": (SOLO_ENV, [("m162_c51", "cta_hbm", 162), ("m555_c90", "cta_hbm", 555), ("m903_c60", "cta_hbm", 903)]),
-    **{f"team{g}": (TEAM_ENV[g], _TEAM) for g in (2, 3, 5)},
+    **{f"team{g}": (TEAM_ENV[g], _TEAM) for g in (1, 2, 3, 5)},
     "team_full": ({}, _TEAM),
-    "tile0": ({"ASAM_TILE_MODE": "0"}, [("team162_c48", "team", 162), ("wide", "team", None)]),
 }
 # device switches read once per process (process-wide __constant__ symbols, statics): these groups run in a subprocess
-SUBPROCESS = {"leaf63", "smem_mma2", "pb_smem24", "tile0"}
+SUBPROCESS = {"leaf63", "smem_mma2", "pb_smem24"}
 # the group that also carries the other kinds of failure (exact zeros, NaNs, two seeds) on one graph of its path
 EXTRA_KINDS = {"leaf": "pendants", "cta_smem": "smem_n51", "cta_hbm": "m555_c90", "team_full": "wide"}
 # pivots of the isolated pose in the valid-range cases, three per 3x3 block, and the prior's residual: at least 1 so
@@ -269,7 +268,7 @@ def test_targets_reach_every_path(built, group):
         # the first columns of the 2nd and 3rd staged panel of 48 / 36 / 24 columns
         assert [staged_width(t.m) for t in ts] == [48, 36, 24]
         assert {36, 72} <= set(by["m555_c90"].cols) and {24, 48} <= set(by["m903_c60"].cols)
-    if group.startswith("team") or group == "tile0":
+    if group.startswith("team"):
         assert {0, 12, 24, 36, 47, 48} <= set(by["wide"].cols) and 96 in by["wide"].cols
         assert by["team162_c48"].c == 48 and by["team162_c48"].cols == [0, 12, 24, 36, 47]
     if group in EXTRA_KINDS:

@@ -18,7 +18,7 @@ END {
   for (f in all) printf("%-70s %6d %6d %6d %6d %6d %6d\n", f, dfma[f], dmma[f], ublk[f], syncs[f], utma[f], tc[f]);
 }' | sort
 echo
-echo "# excerpt from k_factor (tile_rm / tile_mma are non-inlined device functions inside it): mbarrier arm + bulk asynchronous"
+echo "# excerpt from k_factor (tile_rm is a non-inlined device function inside it): mbarrier arm + bulk asynchronous"
 echo "# copies (cp.async.bulk -> UBLKCP.S.G, expect_tx -> SYNCS.ARRIVE.TRANS64, try_wait -> SYNCS.PHASECHK) and the FP64 tensor-pipe"
 echo "# instructions (mma.sync.m8n8k4.f64 -> DMMA.8x8x4)"
 cuobjdump -sass $SO | awk '/Function : _Z8k_factor7FacArgs/ {p=1; next} p && /Function :/ {p=0} p' | grep -E "UBLKCP|SYNCS|DMMA|FENCE\.VIEW|MEMBAR" | sed 's/^ *//' | awk '!seen[$2" "$3]++' | head -40

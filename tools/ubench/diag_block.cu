@@ -143,16 +143,14 @@ int main()
     cudaMemcpy(dA, A.data(), sizeof(double) * n * n, cudaMemcpyHostToDevice);
     int khz = 0; cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);
     std::vector<double> ref(n * n);
-    for (int variant = -1; variant < 4; variant++) {
-        // -1: production code with the DFMA update inside the block; 0: tensor-pipe update (production default);
-        // 1-3: variants / pieces
-        { const int v = variant >= 0; cudaMemcpyToSymbol(g_diag_mma, &v, sizeof(int)); }
-        k_bench<<<1, 256>>>(dA, dO, dS, variant < 0 ? 0 : variant);
+    for (int variant = 0; variant < 4; variant++) {
+        // 0: production code (diag_factor_rl), the reference of the comparison; 1-3: variants / pieces
+        k_bench<<<1, 256>>>(dA, dO, dS, variant);
         cudaError_t e = cudaDeviceSynchronize();
         long long st[10]; std::vector<double> O(n * n);
         cudaMemcpy(st, dS, sizeof(st), cudaMemcpyDeviceToHost);
         cudaMemcpy(O.data(), dO, sizeof(double) * n * n, cudaMemcpyDeviceToHost);
-        if (variant == -1) ref = O;
+        if (variant == 0) ref = O;
         double md = 0;
         for (int j = 0; j < n; j++) for (int i = j; i < n; i++) md = fmax(md, fabs(O[i + j * n] - ref[i + j * n]) / fabs(ref[i + j * n]));
         printf("variant %d: %s  block %lld cycles (%.2f us at %d MHz)  max rel diff vs v0 %.2e\n", variant, cudaGetErrorString(e),
