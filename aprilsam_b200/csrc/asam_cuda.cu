@@ -7,6 +7,7 @@
 
 #include <cuda_runtime.h>
 
+#include <climits>
 #include <cmath>
 #include <cstdarg>
 #include <cstdint>
@@ -1051,7 +1052,7 @@ static int g_world = 1, g_rank = 0, g_sharding = 0;
 #define ASAM_NCCL_FLOAT64 8
 #define ASAM_NCCL_INT32 2
 #define ASAM_NCCL_SUM 0
-#define ASAM_NCCL_MAX 2
+#define ASAM_NCCL_MIN 3
 
 #define NCK(call)                                                                                  \
     do {                                                                                           \
@@ -1233,15 +1234,17 @@ static int shard_exchange(asam_dev *d, int which)
     return 0;
 }
 
-// Sharded solves: a pivot that fails in one rank's shard must fail the solve on EVERY rank (each rank owns a copy of
-// the caller's graph and takes the same action): ctrl[7] = "my status word is non-zero", all-reduced (max); a rank
-// whose own word is clean takes ASAM_STATUS_REMOTE.
+// Sharded solves: every rank reads the same status word, the one of the rank that owns the failure (each rank owns a
+// copy of the caller's graph and takes the same action).  A failed pivot in a shard poisons the shard root's update
+// matrix, which the exchange carries to every rank, so the other ranks fail a top ancestor of it; ancestors have
+// larger ids than their descendants, so the smallest failing supernode is the owner's.  ctrl[7] = the word as a key
+// (timeouts below failed pivots below a clean word), all-reduced (min), written back.
 __global__ void k_status_flag(int *ctrl, int phase)
 {
     if (phase == 0)
-        ctrl[7] = ctrl[1] != 0;
-    else if (ctrl[7] != 0 && ctrl[1] == 0)
-        ctrl[1] = ASAM_STATUS_REMOTE;
+        ctrl[7] = ctrl[1] == 0 ? INT_MAX : ctrl[1];
+    else
+        ctrl[1] = ctrl[7] == INT_MAX ? 0 : ctrl[7];
 }
 
 static int shard_status_agree(asam_dev *d)
@@ -1250,7 +1253,7 @@ static int shard_status_agree(asam_dev *d)
         return 0;
     int *ctrl = (int *) d->ctrl.p;
     k_status_flag<<<1, 1, 0, d->stream>>>(ctrl, 0);
-    NCK(g_nccl.AllReduce(ctrl + 7, ctrl + 7, 1, ASAM_NCCL_INT32, ASAM_NCCL_MAX, g_comm, d->stream));
+    NCK(g_nccl.AllReduce(ctrl + 7, ctrl + 7, 1, ASAM_NCCL_INT32, ASAM_NCCL_MIN, g_comm, d->stream));
     k_status_flag<<<1, 1, 0, d->stream>>>(ctrl, 1);
     CK(cudaGetLastError());
     d->n_launch += 3;

@@ -673,9 +673,6 @@ static void report_factor_status(solver_t *s, int status, const char *where)
         s->hdr.is_spd = 0;
         asam_fatal("%s: information matrix is not positive definite (pivot <= 0 in supernode %d)", where,
                    status - 1);
-    } else if (status == ASAM_STATUS_REMOTE) {
-        s->hdr.is_spd = 0;
-        asam_fatal("%s: another rank of the sharded solve reported a failed factorisation (not positive definite?)", where);
     } else if (status < 0) {
         asam_fatal("%s: internal scheduling error in the factorisation kernel (supernode %d)", where, -status - 1);
     }

@@ -179,9 +179,9 @@ int asam_chi2(asam_dev_t *d, int n_factors, double *chi2_out);
  * <0 = internal dependency timeout.  A failed pivot turns its ancestors NaN, but they start only after their
  * children have arrived, so with one failure the status names the FIRST failing supernode, never an ancestor;
  * failures in disjoint subtrees report one of them.  A non-zero status, once read, resets the control words,
- * so the context can factor again (tests/test_gpu_pivots.py); ASAM_STATUS_REMOTE = another rank of a sharded solve failed (the ranks agree
- * on failure before the status is read, so that all of them take the same action). */
-#define ASAM_STATUS_REMOTE (-(1 << 28))
+ * so the context can factor again (tests/test_gpu_pivots.py).  In a sharded solve every rank reads the same word, the
+ * owner's: a failure in one rank's shard names that shard's supernode on every rank, and a timeout on any rank is a
+ * timeout on every rank (tests/test_gpu_sharded.py). */
 int asam_factor_status(asam_dev_t *d, int *status_out);
 
 /* Debug / test access (not used on the solve path). */
