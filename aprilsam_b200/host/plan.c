@@ -392,7 +392,7 @@ static int front_fits_smem(int mb)
 
 /* Fronts up to this order that do not fit in shared memory go to ONE CTA (cta_front's HBM mode) even where
  * their team would be larger; by default (0) only the fronts whose team the level room scales below two CTAs do
- * (build_schedule).  ASAM_SOLO_MAX_M overrides (tuning). */
+ * (team_sizes).  ASAM_SOLO_MAX_M overrides (tuning). */
 static int solo_max_m(void)
 {
     static int v = -1;
@@ -403,11 +403,13 @@ static int solo_max_m(void)
     return v;
 }
 
+/* Returns the team word of a front, the G field of its task word (pack_nwait): 0 = one CTA on cta_front,
+ * >= 2 = a team of G CTAs (team_front); team_sizes() may also scale a team to 1 = team_front on one CTA. */
 static int team_size(int mb, int cb, int cap)
 {
     int64_t m = 3 * (int64_t) mb, c = 3 * (int64_t) cb;
     if (front_fits_smem(mb) || m <= solo_max_m())
-        return 1;
+        return 0;
     int64_t j0 = c < 48 ? c : 48, tiles = 0;
     for (int64_t cb0 = j0; cb0 < m; cb0 += 64)
         tiles += (m - cb0 + 1 + 255) / 256;
@@ -443,6 +445,9 @@ static inline int pack_nwait(int nw, int w, int G)
     return (nw & 0xffff) | (w << 16) | (G << 24);
 }
 
+/* CTAs (= consecutive task entries) of a front of team word G */
+static inline int front_ctas(int G) { return G > 1 ? G : 1; }
+
 static int plan_team_cap(const plan_t *pl) { return pl->max_team > 0 ? pl->max_team : 120; }
 
 /* doubles of the arena a front of mb block rows occupies: the front itself and, for fronts that do not fit
@@ -454,8 +459,8 @@ static int64_t front_doubles(int mb)
 }
 
 /* ---- schedule: task lists of one batch solve ------------------------------------------------
- * Single GPU (world == 1): leaf set -> k_factor_leaf, everything else -> k_factor (level order,
- * teams expanded), back-solve list = [rest | leaf set], parents first.
+ * Single GPU (world == 1): leaf set -> k_factor_leaf, everything else -> k_factor (ticket order of
+ * factor_order(), teams expanded), back-solve list = [rest | leaf set], parents first.
  *
  * Several GPUs (world > 1, one process each, SURVEY.md section 8e): the elimination tree is cut into
  * disjoint subtrees ("shards") that are dealt to the ranks; a rank factors its own shards (same
@@ -503,6 +508,20 @@ static int cmp_key_desc(const void *a, const void *b)
     return (x->id > y->id) - (x->id < y->id); /* deterministic */
 }
 
+/* out[0 .. n) = 0 .. n-1 by descending key, ties by ascending id */
+static void order_desc(const double *key, int n, int *out)
+{
+    sn_key_t *keys = malloc(sizeof(sn_key_t) * (size_t) (n + 1));
+    for (int s = 0; s < n; s++) {
+        keys[s].key = key[s];
+        keys[s].id = s;
+    }
+    qsort(keys, (size_t) n, sizeof(sn_key_t), cmp_key_desc);
+    for (int k = 0; k < n; k++)
+        out[k] = keys[k].id;
+    free(keys);
+}
+
 /* Modelled duration (microseconds) of front s once its children are done, factored by g CTAs (least-squares
  * fits to device traces of the 100 k world, tools/panel_trace.py --dump-trace).  ASAM_TEAM_MODEL="a,b,c,d,e"
  * overrides the team coefficients (tuning).  A fit to H100 traces of the current team path (children ready ->
@@ -521,7 +540,7 @@ static void team_model_init(void)
         sscanf(e, "%lf,%lf,%lf,%lf,%lf", &team_model[0], &team_model[1], &team_model[2], &team_model[3], &team_model[4]);
 }
 
-/* g: the team size, 0 for one CTA on cta_front */
+/* g: the team word (team_size()) */
 static double front_lat_us(const plan_t *pl, int s, int g)
 {
     const double m = 3.0 * pl->desc[s].mb, c = 3.0 * pl->desc[s].cb;
@@ -598,7 +617,7 @@ static hp_t hp_pop(hp_t *h, int *n, int maxheap)
 }
 
 /* returns the number of entries written to out[] (= tasks with in[s] != 0) */
-static int sim_order(const plan_t *pl, const char *in, const int *G_of, const double *lat, const double *prio, int P, int *out)
+static int sim_order(const plan_t *pl, const char *in, const int *G, const double *lat, const double *prio, int P, int *out)
 {
     const int nsn = pl->nsn;
     int *pending = calloc((size_t) nsn + 1, sizeof(int));
@@ -613,7 +632,7 @@ static int sim_order(const plan_t *pl, const char *in, const int *G_of, const do
     double now = 0.0;
     for (;;) {
         while (nready > 0) {
-            int s = ready[0].id, g = G_of[s] < 0 ? 1 : (G_of[s] > P ? P : G_of[s]);
+            int s = ready[0].id, g = front_ctas(G[s]) < P ? front_ctas(G[s]) : P;
             if (g > free_cta && nev > 0)
                 break; /* tickets are strictly ordered: nothing overtakes a team that is gathering its CTAs */
             hp_pop(ready, &nready, 1);
@@ -626,7 +645,7 @@ static int sim_order(const plan_t *pl, const char *in, const int *G_of, const do
         hp_t e = hp_pop(events, &nev, 0);
         now = e.key;
         {
-            int s = e.id, g = G_of[s] < 0 ? 1 : (G_of[s] > P ? P : G_of[s]);
+            int s = e.id, g = front_ctas(G[s]) < P ? front_ctas(G[s]) : P;
             free_cta += g;
             if (free_cta > P)
                 free_cta = P;
@@ -641,403 +660,371 @@ static int sim_order(const plan_t *pl, const char *in, const int *G_of, const do
     return nout;
 }
 
-static void build_schedule(plan_t *pl)
+/* owner[s]: rank that factors s, -1 = top (every rank).  Several ranks: the cut and the shard descriptors of pl. */
+static int *shard_cut(plan_t *pl, int W)
 {
-    const int nsn = pl->nsn, W = pl->world > 1 ? pl->world : 1, me = pl->world > 1 ? pl->rank : 0;
-    free(pl->tasks); free(pl->nwait); free(pl->btasks); free(pl->leaf_tasks);
-    free(pl->top_tasks); free(pl->top_nwait);
+    const int nsn = pl->nsn;
     free(pl->shard_owner); free(pl->shard_off); free(pl->shard_cnt); free(pl->shard_q0); free(pl->shard_qn);
-    pl->top_tasks = pl->top_nwait = pl->shard_owner = pl->shard_q0 = pl->shard_qn = NULL;
+    pl->shard_owner = pl->shard_q0 = pl->shard_qn = NULL;
     pl->shard_off = pl->shard_cnt = NULL;
-    pl->n_top = pl->n_top_sn = pl->n_shards = 0;
-
-    /* owner[s]: rank that factors s, -1 = top (every rank) */
-    int *owner = malloc(sizeof(int) * (size_t) (nsn + 1));
+    pl->n_shards = 0;
+    int *owner = calloc((size_t) nsn + 1, sizeof(int));
+    if (W <= 1 || nsn == 0)
+        return owner;
+    double *sub = malloc(sizeof(double) * (size_t) nsn); /* work of the subtree rooted at s */
     for (int s = 0; s < nsn; s++)
-        owner[s] = 0;
-    if (W > 1 && nsn > 0) {
-        double *sub = malloc(sizeof(double) * (size_t) nsn); /* work of the subtree rooted at s */
-        for (int s = 0; s < nsn; s++)
-            sub[s] = sn_work(&pl->desc[s]);
-        for (int s = 0; s < nsn; s++) /* children have smaller ids */
-            if (pl->desc[s].parent >= 0)
-                sub[pl->desc[s].parent] += sub[s];
-        /* frontier of subtree roots; split the heaviest until the shards can be balanced */
-        int *fr = malloc(sizeof(int) * (size_t) (nsn + 1)), nfr = 0;
-        double total = 0.0;
-        for (int s = 0; s < nsn; s++)
-            if (pl->desc[s].parent < 0) {
-                fr[nfr++] = s;
-                total += sub[s];
+        sub[s] = sn_work(&pl->desc[s]);
+    for (int s = 0; s < nsn; s++) /* children have smaller ids */
+        if (pl->desc[s].parent >= 0)
+            sub[pl->desc[s].parent] += sub[s];
+    /* frontier of subtree roots; split the heaviest until the shards can be balanced */
+    int *fr = malloc(sizeof(int) * (size_t) (nsn + 1)), nfr = 0;
+    for (int s = 0; s < nsn; s++)
+        if (pl->desc[s].parent < 0)
+            fr[nfr++] = s;
+    for (int s = 0; s < nsn; s++)
+        owner[s] = -2; /* undecided */
+    const int max_shards = 16 * W;
+    /* ASAM_SHARD_TOL: imbalance at which the splitting stops (tuning).  Every split moves one more front of the
+     * dependent chain above the cut, where all ranks repeat it */
+    const double shard_tol = getenv("ASAM_SHARD_TOL") ? atof(getenv("ASAM_SHARD_TOL")) : ASAM_SHARD_TOL_DEFAULT;
+    double *load = malloc(sizeof(double) * (size_t) W);
+    for (;;) {
+        /* heaviest-first dealing (LPT) of the current frontier */
+        for (int i = 1; i < nfr; i++) { /* insertion sort by (work desc, id asc): deterministic */
+            int v = fr[i], j = i - 1;
+            while (j >= 0 && (sub[fr[j]] < sub[v] || (sub[fr[j]] == sub[v] && fr[j] > v))) {
+                fr[j + 1] = fr[j];
+                j--;
             }
-        for (int s = 0; s < nsn; s++)
-            owner[s] = -2; /* undecided */
-        const int max_shards = 16 * W;
-        /* ASAM_SHARD_TOL: imbalance at which the splitting stops (tuning).  Every split moves one more front of the
-         * dependent chain above the cut, where all ranks repeat it */
-        const double shard_tol = getenv("ASAM_SHARD_TOL") ? atof(getenv("ASAM_SHARD_TOL")) : ASAM_SHARD_TOL_DEFAULT;
-        double *load = malloc(sizeof(double) * (size_t) W);
-        for (;;) {
-            /* heaviest-first dealing (LPT) of the current frontier */
-            for (int i = 1; i < nfr; i++) { /* insertion sort by (work desc, id asc): deterministic */
-                int v = fr[i], j = i - 1;
-                while (j >= 0 && (sub[fr[j]] < sub[v] || (sub[fr[j]] == sub[v] && fr[j] > v))) {
-                    fr[j + 1] = fr[j];
-                    j--;
-                }
-                fr[j + 1] = v;
-            }
-            for (int r = 0; r < W; r++)
-                load[r] = 0.0;
-            double shard_sum = 0.0;
-            for (int i = 0; i < nfr; i++) {
-                int best = 0;
-                for (int r = 1; r < W; r++)
-                    if (load[r] < load[best])
-                        best = r;
-                load[best] += sub[fr[i]];
-                shard_sum += sub[fr[i]];
-            }
-            double mx = 0.0;
-            for (int r = 0; r < W; r++)
-                if (load[r] > mx)
-                    mx = load[r];
-            /* stop when balanced within 10 %, when there are plenty of shards, or when the heaviest
-             * shard cannot be split (no children) */
-            int h = fr[0];
-            if (nfr >= W && mx <= shard_tol * shard_sum / W)
-                break;
-            if (nfr >= max_shards || pl->snh[h].children.n == 0)
-                break;
-            owner[h] = -1; /* the root of the heaviest shard moves above the cut */
-            fr[0] = fr[nfr - 1];
-            nfr--;
-            for (int c = 0; c < pl->snh[h].children.n; c++)
-                fr[nfr++] = pl->snh[h].children.p[c];
+            fr[j + 1] = v;
         }
-        /* final dealing + shard descriptors */
         for (int r = 0; r < W; r++)
             load[r] = 0.0;
-        pl->n_shards = nfr;
-        pl->shard_owner = malloc(sizeof(int) * (size_t) (nfr + 1));
-        pl->shard_off = malloc(sizeof(int64_t) * (size_t) (nfr + 1));
-        pl->shard_cnt = malloc(sizeof(int64_t) * (size_t) (nfr + 1));
-        pl->shard_q0 = malloc(sizeof(int) * (size_t) (nfr + 1));
-        pl->shard_qn = malloc(sizeof(int) * (size_t) (nfr + 1));
-        int *npose = calloc((size_t) nsn + 1, sizeof(int)); /* poses in the subtree of s */
-        for (int s = 0; s < nsn; s++) {
-            npose[s] += pl->desc[s].cb;
-            if (pl->desc[s].parent >= 0)
-                npose[pl->desc[s].parent] += npose[s];
-        }
+        double shard_sum = 0.0;
         for (int i = 0; i < nfr; i++) {
-            int best = 0, s = fr[i];
+            int best = 0;
             for (int r = 1; r < W; r++)
                 if (load[r] < load[best])
                     best = r;
-            load[best] += sub[s];
-            owner[s] = best;
-            const asam_sn_desc_t *d = &pl->desc[s];
-            int64_t m = 3 * (int64_t) d->mb, c = 3 * (int64_t) d->cb, ld = ASAM_LD(m);
-            pl->shard_owner[i] = best;
-            pl->shard_off[i] = d->f_off + c * ld;   /* trailing columns: update matrix + rhs row */
-            pl->shard_cnt[i] = (m - c) * ld;
-            pl->shard_qn[i] = npose[s];
-            pl->shard_q0[i] = d->first + d->cb - npose[s];
+            load[best] += sub[fr[i]];
+            shard_sum += sub[fr[i]];
         }
-        /* push ownership down the shards (parents have larger ids) */
-        for (int s = nsn - 1; s >= 0; s--)
-            if (owner[s] == -2)
-                owner[s] = pl->desc[s].parent >= 0 ? owner[pl->desc[s].parent] : -1;
-        free(npose);
-        free(load);
-        free(fr);
-        free(sub);
+        double mx = 0.0;
+        for (int r = 0; r < W; r++)
+            if (load[r] > mx)
+                mx = load[r];
+        /* stop when balanced within 10 %, when there are plenty of shards, or when the heaviest
+         * shard cannot be split (no children) */
+        int h = fr[0];
+        if (nfr >= W && mx <= shard_tol * shard_sum / W)
+            break;
+        if (nfr >= max_shards || pl->snh[h].children.n == 0)
+            break;
+        owner[h] = -1; /* the root of the heaviest shard moves above the cut */
+        fr[0] = fr[nfr - 1];
+        nfr--;
+        for (int c = 0; c < pl->snh[h].children.n; c++)
+            fr[nfr++] = pl->snh[h].children.p[c];
     }
+    /* final dealing + shard descriptors */
+    for (int r = 0; r < W; r++)
+        load[r] = 0.0;
+    pl->n_shards = nfr;
+    pl->shard_owner = malloc(sizeof(int) * (size_t) (nfr + 1));
+    pl->shard_off = malloc(sizeof(int64_t) * (size_t) (nfr + 1));
+    pl->shard_cnt = malloc(sizeof(int64_t) * (size_t) (nfr + 1));
+    pl->shard_q0 = malloc(sizeof(int) * (size_t) (nfr + 1));
+    pl->shard_qn = malloc(sizeof(int) * (size_t) (nfr + 1));
+    int *npose = calloc((size_t) nsn + 1, sizeof(int)); /* poses in the subtree of s */
+    for (int s = 0; s < nsn; s++) {
+        npose[s] += pl->desc[s].cb;
+        if (pl->desc[s].parent >= 0)
+            npose[pl->desc[s].parent] += npose[s];
+    }
+    for (int i = 0; i < nfr; i++) {
+        int best = 0, s = fr[i];
+        for (int r = 1; r < W; r++)
+            if (load[r] < load[best])
+                best = r;
+        load[best] += sub[s];
+        owner[s] = best;
+        const asam_sn_desc_t *d = &pl->desc[s];
+        int64_t m = 3 * (int64_t) d->mb, c = 3 * (int64_t) d->cb, ld = ASAM_LD(m);
+        pl->shard_owner[i] = best;
+        pl->shard_off[i] = d->f_off + c * ld;   /* trailing columns: update matrix + rhs row */
+        pl->shard_cnt[i] = (m - c) * ld;
+        pl->shard_qn[i] = npose[s];
+        pl->shard_q0[i] = d->first + d->cb - npose[s];
+    }
+    /* push ownership down the shards (parents have larger ids) */
+    for (int s = nsn - 1; s >= 0; s--)
+        if (owner[s] == -2)
+            owner[s] = pl->desc[s].parent >= 0 ? owner[pl->desc[s].parent] : -1;
+    free(npose);
+    free(load);
+    free(fr);
+    free(sub);
+    return owner;
+}
 
-    /* leaf set: supernodes whose whole subtree consists of fronts small enough for the
+/* Returns the factor leaf set; sets the back-solve leaf set (pl->bs_leaf, pl->n_bs_leaf). */
+static char *leaf_sets(plan_t *pl, const int *owner, int me)
+{
+    const int nsn = pl->nsn;
+    /* factor leaf set: supernodes whose whole subtree consists of fronts small enough for the
      * warp-per-front kernels (children have smaller ids).  Only worth separate launches when
      * there are thousands of them. */
     char *leaf = calloc((size_t) nsn + 1, 1);
-    int n_leaf_all = 0;
+    int n_leaf = 0;
     const int leaf_max = leaf_max_m_for(nsn);
     for (int s = 0; s < nsn; s++) {
         int ok = 3 * pl->desc[s].mb <= leaf_max;
         for (int c = 0; ok && c < pl->snh[s].children.n; c++)
             ok = leaf[pl->snh[s].children.p[c]];
         leaf[s] = (char) ok;
-        n_leaf_all += ok;
+        n_leaf += ok;
     }
-    if (n_leaf_all < ASAM_LEAF_MIN_COUNT)
+    if (n_leaf < ASAM_LEAF_MIN_COUNT)
         memset(leaf, 0, (size_t) nsn);
     /* the warp-per-supernode BACK-SOLVE takes any downward-closed set with <= 64 own columns and
      * <= 64 rows below (a superset of the factor leaf set); it pays from a few dozen supernodes on:
      * a warp per supernode has everything fetched before its parent's flag arrives */
     free(pl->bs_leaf);
     pl->bs_leaf = calloc((size_t) pl->sn_cap + 1, 1);
+    int n_bsl = 0;
     for (int s = 0; s < nsn; s++) {
         int ok = 3 * pl->desc[s].cb <= ASAM_BSLEAF_MAX && 3 * (pl->desc[s].mb - pl->desc[s].cb) <= ASAM_BSLEAF_MAX;
         for (int c = 0; ok && c < pl->snh[s].children.n; c++)
             ok = pl->bs_leaf[pl->snh[s].children.p[c]];
         pl->bs_leaf[s] = (char) ok;
+        n_bsl += ok && owner[s] == me;
     }
-
-    /* Task order.  The persistent kernels hand out tasks in list order, so the list IS the schedule.  Plain
-     * level order (every front of level l before any of level l+1) starts the deepest chain of the tree last
-     * among its level-mates and leaves its top to run alone at the end, with most SMs spinning.
-     * Critical-path-first instead: fronts are listed by
-     * DESCENDING length of the dependent chain from them up to the root (their own modelled latency
-     * included), which is still a topological order -- a child's chain is its parent's plus its own -- so a
-     * waiting CTA only ever waits for tasks that were handed out before its own.  ASAM_TASK_ORDER=level keeps
-     * the level order (A/B). */
-    int *byl = malloc(sizeof(int) * (size_t) (nsn + 1));
-    int order_mode = 0; /* 0 level, 1 chain length ("cp"), 2 simulated schedule ("sim"), 3 auto: cp or sim by load */
-    int *bylv = malloc(sizeof(int) * (size_t) (nsn + 1)); /* plain level order: the back-substitution list (faster
-                                                            * than the reversed chain order in A/B runs) */
-    {
-        int *cnt = calloc((size_t) pl->n_levels + 2, sizeof(int));
-        for (int s = 0; s < nsn; s++)
-            cnt[pl->desc[s].level + 1]++;
-        for (int l = 0; l < pl->n_levels; l++)
-            cnt[l + 1] += cnt[l];
-        for (int s = 0; s < nsn; s++)
-            bylv[cnt[pl->desc[s].level]++] = s;
-        free(cnt);
-    }
-    {
-        const char *eo = getenv("ASAM_TASK_ORDER");
-        if (eo && strcmp(eo, "level") == 0) {
-            memcpy(byl, bylv, sizeof(int) * (size_t) nsn);
-        } else {
-            order_mode = (eo && strcmp(eo, "cp") == 0) ? 1 : ((eo && strcmp(eo, "sim") == 0) ? 2 : 3);
-        }
-    }
-
-    /* team sizes.  A front's team is bound by latency, not throughput (team_size()), so where one tree
-     * level holds more team fronts than the SMs can seat side by side, smaller teams finish the
-     * LEVEL sooner: CTA-time per front (G x duration) falls with G.  Scale the teams of such a level
-     * down to the room there is (never below 2). */
-    int *G_of = malloc(sizeof(int) * (size_t) (nsn + 1));
-    {
-        int64_t *want = calloc((size_t) pl->n_levels + 1, sizeof(int64_t));
-        for (int s = 0; s < nsn; s++) {
-            G_of[s] = (owner[s] == me || owner[s] == -1) && !leaf[s] ? team_size(pl->desc[s].mb, pl->desc[s].cb, plan_team_cap(pl)) : 1;
-            if (G_of[s] > 1)
-                want[pl->desc[s].level] += G_of[s];
-        }
-        int64_t room = ASAM_TEAM_ROOM < plan_team_cap(pl) ? ASAM_TEAM_ROOM : plan_team_cap(pl);
-        const char *er = getenv("ASAM_TEAM_ROOM"); /* tuning knob (tools only) */
-        if (er && atoi(er) > 0)
-            room = atoi(er);
-        /* A front scaled below a team of two is factored by ONE CTA on cta_front's HBM path (task word G = 0): it
-         * pays where a level holds far more team fronts than SMs (the SM time per front is what limits the level,
-         * not its latency), and one CTA needs none of the team protocol.  ASAM_TEAM_MIN=g (A/B) sets the smallest
-         * team instead; with g = 1 such fronts run the team code alone (G = 1). */
-        int gmin = 0;
-        const char *em = getenv("ASAM_TEAM_MIN");
-        if (em && atoi(em) >= 1)
-            gmin = atoi(em);
-        for (int s = 0; s < nsn; s++) {
-            int64_t w = want[pl->desc[s].level];
-            if (G_of[s] > 1 && w > room) {
-                int g = (int) ((int64_t) G_of[s] * room / w);
-                g = g < gmin ? gmin : g;
-                G_of[s] = g >= 2 ? g : (gmin == 1 ? -1 : 1); /* -1: one CTA, team code path */
-            }
-        }
-        free(want);
-    }
-    if (order_mode != 0) {
-        /* modelled duration of every front once its children are done (microseconds; least-squares fit to device
-         * traces of the 100 k world, tools/panel_trace.py --dump-trace: median error 8 % for shared-memory fronts,
-         * 9 % for teams) and the length of the dependent chain from a front up to the root */
-        double *lat_us = malloc(sizeof(double) * (size_t) (nsn + 1)), *up_us = malloc(sizeof(double) * (size_t) (nsn + 1));
-        double work = 0.0, chain = 0.0;
-        team_model_init();
-        for (int s = nsn - 1; s >= 0; s--) { /* parents have larger ids */
-            const int g = G_of[s] < 0 ? 1 : G_of[s];
-            const double lat = front_lat_us(pl, s, G_of[s] == 1 ? 0 : g);
-            lat_us[s] = lat;
-            up_us[s] = lat + (pl->desc[s].parent >= 0 ? up_us[pl->desc[s].parent] : 0.0);
-            if ((owner[s] == me || owner[s] == -1) && !leaf[s])
-                work += lat * g;
-            if (up_us[s] > chain)
-                chain = up_us[s];
-        }
-        const int P = pl->n_cta > 0 ? pl->n_cta : 132;
-        /* auto: where the SMs are far from saturated (M3500: 11 of 67 CTA-ms busy) spinning costs nothing and the
-         * eager chain-length order starts parents soonest; where they are saturated, a team must not take its
-         * CTAs before it can use them */
-        const int use_sim = order_mode == 2 || (order_mode == 3 && work / P > 0.5 * chain);
-        {
-            sn_key_t *keys = malloc(sizeof(sn_key_t) * (size_t) (nsn + 1));
-            for (int s = 0; s < nsn; s++) {
-                keys[s].key = up_us[s];
-                keys[s].id = s;
-            }
-            qsort(keys, (size_t) nsn, sizeof(sn_key_t), cmp_key_desc);
-            for (int k = 0; k < nsn; k++)
-                byl[k] = keys[k].id;
-            free(keys);
-        }
-        if (use_sim) {
-            /* ticket order of k_factor = start order of the simulated schedule; the main list (own fronts outside
-             * the leaf set) and the part above a multi-GPU cut are separate launches, simulated separately; the
-             * leaf set keeps the chain-length order (warp-sized tasks: nothing to gather) */
-            char *in = calloc((size_t) nsn + 1, 1);
-            int *ord = malloc(sizeof(int) * (size_t) (nsn + 1)), *pos_of = malloc(sizeof(int) * (size_t) (nsn + 1));
-            int n1, n2;
-            for (int s = 0; s < nsn; s++)
-                in[s] = owner[s] == me && !leaf[s];
-            n1 = sim_order(pl, in, G_of, lat_us, up_us, P, ord);
-            for (int s = 0; s < nsn; s++)
-                in[s] = owner[s] == -1;
-            n2 = sim_order(pl, in, G_of, lat_us, up_us, P, ord + n1);
-            for (int s = 0; s < nsn; s++)
-                pos_of[s] = -1;
-            for (int k = 0; k < n1 + n2; k++)
-                pos_of[ord[k]] = k;
-            /* byl: simulated tasks in start order, everything else (leaf set, other ranks) after them in the old order */
-            int *nb = malloc(sizeof(int) * (size_t) (nsn + 1)), k2 = 0;
-            for (int k = 0; k < n1 + n2; k++)
-                nb[k2++] = ord[k];
-            for (int k = 0; k < nsn; k++)
-                if (pos_of[byl[k]] < 0)
-                    nb[k2++] = byl[k];
-            memcpy(byl, nb, sizeof(int) * (size_t) nsn);
-            free(nb);
-            free(in);
-            free(ord);
-            free(pos_of);
-        }
-        free(lat_us);
-        free(up_us);
-    }
-
-    /* Back-solve entries of a supernode: one, or -- supernodes wider than one 96-column block (ASAM_BSW) in a
-     * batch schedule -- one per block, last block first, each solved by its own CTA (cta_backsolve, blk_only).
-     * Entry word: supernode | (block + 1) << 24.  ASAM_BS_SPLIT=0 switches the split off (A/B). */
-    int bs_split = 1;
-    {
-        const char *eb = getenv("ASAM_BS_SPLIT");
-        if (eb)
-            bs_split = atoi(eb) != 0;
-    }
-    pl->bt_split = 0;
-#define BS_NBLK(s_) ((bs_split && !pl->bs_leaf[s_] && 3 * pl->desc[s_].cb > 96 && pl->nsn < (1 << 24)) ? (3 * pl->desc[s_].cb + 95) / 96 : 1)
-    int64_t n_local = 0, n_top = 0;
-    int n_leaf = 0, n_main_sn = 0, n_top_sn = 0, n_bsl = 0, n_top_bt = 0;
-    for (int s = 0; s < nsn; s++)
-        n_bsl += owner[s] == me && pl->bs_leaf[s];
     if (n_bsl < ASAM_BSLEAF_MIN_COUNT) {
         memset(pl->bs_leaf, 0, (size_t) nsn);
         n_bsl = 0;
     }
+    pl->n_bs_leaf = n_bsl;
+    return leaf;
+}
+
+/* Team word of every supernode (team_size(); 0 for the leaf set and other ranks' fronts).  A front's team is bound
+ * by latency, not throughput (team_size()), so where one tree level holds more team fronts than the SMs can seat
+ * side by side, smaller teams finish the LEVEL sooner: CTA-time per front (G x duration) falls with G.  The teams of
+ * such a level are scaled down to the room there is. */
+static int *team_sizes(const plan_t *pl, const int *owner, int me, const char *leaf)
+{
+    const int nsn = pl->nsn;
+    int *G = malloc(sizeof(int) * (size_t) (nsn + 1));
+    int64_t *want = calloc((size_t) pl->n_levels + 1, sizeof(int64_t));
+    for (int s = 0; s < nsn; s++) {
+        G[s] = (owner[s] == me || owner[s] == -1) && !leaf[s] ? team_size(pl->desc[s].mb, pl->desc[s].cb, plan_team_cap(pl)) : 0;
+        if (G[s] >= 2)
+            want[pl->desc[s].level] += G[s];
+    }
+    int64_t room = ASAM_TEAM_ROOM < plan_team_cap(pl) ? ASAM_TEAM_ROOM : plan_team_cap(pl);
+    const char *er = getenv("ASAM_TEAM_ROOM"); /* tuning knob (tools only) */
+    if (er && atoi(er) > 0)
+        room = atoi(er);
+    /* A front scaled below a team of two is factored by ONE CTA on cta_front's HBM path (word 0): it pays where a
+     * level holds far more team fronts than SMs (the SM time per front is what limits the level, not its latency),
+     * and one CTA needs none of the team protocol.  ASAM_TEAM_MIN=g (A/B) sets the smallest team instead; with
+     * g = 1 such fronts run the team code alone (word 1). */
+    int gmin = 0;
+    const char *em = getenv("ASAM_TEAM_MIN");
+    if (em && atoi(em) >= 1)
+        gmin = atoi(em);
+    for (int s = 0; s < nsn; s++) {
+        int64_t w = want[pl->desc[s].level];
+        if (G[s] >= 2 && w > room) {
+            int g = (int) ((int64_t) G[s] * room / w);
+            g = g < gmin ? gmin : g;
+            G[s] = g >= 2 || gmin == 1 ? g : 0;
+        }
+    }
+    free(want);
+    return G;
+}
+
+/* Ticket order of k_factor (returned: every supernode once; the task lists take theirs in this order).  The
+ * persistent kernels hand out tasks in list order, so the list IS the schedule.  Plain level order (every front
+ * of level l before any of level l+1) starts the deepest chain of the tree last among its level-mates and leaves
+ * its top to run alone at the end, with most SMs spinning.  Critical-path-first instead ("cp"): fronts are listed
+ * by DESCENDING length of the dependent chain from them up to the root (their own modelled latency included),
+ * which is still a topological order -- a child's chain is its parent's plus its own -- so a waiting CTA only ever
+ * waits for tasks that were handed out before its own.  Where the SMs are saturated, the simulated schedule
+ * ("sim", sim_order()) instead.  ASAM_TASK_ORDER=cp|sim forces one of the two. */
+static int *factor_order(const plan_t *pl, const int *owner, int me, const char *leaf, const int *G)
+{
+    const int nsn = pl->nsn;
+    const char *eo = getenv("ASAM_TASK_ORDER");
+    const int force_cp = eo && strcmp(eo, "cp") == 0, force_sim = eo && strcmp(eo, "sim") == 0;
+    /* modelled duration of every front once its children are done (microseconds; least-squares fit to device
+     * traces of the 100 k world, tools/panel_trace.py --dump-trace: median error 8 % for shared-memory fronts,
+     * 9 % for teams) and the length of the dependent chain from a front up to the root */
+    double *lat_us = malloc(sizeof(double) * (size_t) (nsn + 1)), *up_us = malloc(sizeof(double) * (size_t) (nsn + 1));
+    double work = 0.0, chain = 0.0;
+    team_model_init();
+    for (int s = nsn - 1; s >= 0; s--) { /* parents have larger ids */
+        const double lat = front_lat_us(pl, s, G[s]);
+        lat_us[s] = lat;
+        up_us[s] = lat + (pl->desc[s].parent >= 0 ? up_us[pl->desc[s].parent] : 0.0);
+        if ((owner[s] == me || owner[s] == -1) && !leaf[s])
+            work += lat * front_ctas(G[s]);
+        if (up_us[s] > chain)
+            chain = up_us[s];
+    }
+    const int P = pl->n_cta > 0 ? pl->n_cta : 132;
+    /* auto: where the SMs are far from saturated (M3500: 11 of 67 CTA-ms busy) spinning costs nothing and the
+     * eager chain-length order starts parents soonest; where they are saturated, a team must not take its
+     * CTAs before it can use them */
+    const int use_sim = force_sim || (!force_cp && work / P > 0.5 * chain);
+    int *ord = malloc(sizeof(int) * (size_t) (nsn + 1));
+    order_desc(up_us, nsn, ord);
+    if (use_sim) {
+        /* ticket order of k_factor = start order of the simulated schedule; the main list (own fronts outside
+         * the leaf set) and the part above a multi-GPU cut are separate launches, simulated separately; the
+         * leaf set keeps the chain-length order (warp-sized tasks: nothing to gather) */
+        char *in = calloc((size_t) nsn + 1, 1);
+        int *sim = malloc(sizeof(int) * (size_t) (nsn + 1)), n;
+        for (int s = 0; s < nsn; s++)
+            in[s] = owner[s] == me && !leaf[s];
+        n = sim_order(pl, in, G, lat_us, up_us, P, sim);
+        for (int s = 0; s < nsn; s++)
+            in[s] = owner[s] == -1;
+        n += sim_order(pl, in, G, lat_us, up_us, P, sim + n);
+        /* simulated tasks in start order, everything else (leaf set, other ranks) after them in chain-length order */
+        memset(in, 0, (size_t) nsn);
+        for (int k = 0; k < n; k++)
+            in[sim[k]] = 1;
+        for (int k = 0; k < nsn; k++)
+            if (!in[ord[k]])
+                sim[n++] = ord[k];
+        free(ord);
+        free(in);
+        ord = sim;
+    }
+    free(lat_us);
+    free(up_us);
+    return ord;
+}
+
+/* Back-solve order (returned), parents first: by the modelled TIME of the longest chain below a supernode (its own
+ * solve included), longest first -- a parent's chain is longer than any child's, so the order is topological, and
+ * the deep chains do not queue behind the thousands of supernodes that merely share their height (level order: the
+ * bottom of the longest chain of the 100 k world got its tickets late at every link). */
+static int *backsolve_order(const plan_t *pl)
+{
+    const int nsn = pl->nsn;
+    double *down = calloc((size_t) nsn + 1, sizeof(double));
+    int *ord = malloc(sizeof(int) * (size_t) (nsn + 1));
+    for (int s = 0; s < nsn; s++) { /* children have smaller ids: down[s] holds max over children here */
+        if (!pl->bs_leaf[s]) /* (the warp-per-supernode set runs in a launch of its own, afterwards) */
+            down[s] += 5.0 + 0.17 * 3.0 * pl->desc[s].cb + 0.01 * 3.0 * pl->desc[s].mb;
+        else
+            down[s] += 1e-3 * (pl->desc[s].level + 1);
+        const int par = pl->desc[s].parent;
+        if (par >= 0 && down[s] > down[par])
+            down[par] = down[s];
+    }
+    order_desc(down, nsn, ord);
+    free(down);
+    return ord;
+}
+
+/* Back-solve entries of a supernode in a batch schedule: one, or -- supernodes wider than one 96-column block
+ * (ASAM_BSW) -- one per block, each solved by its own CTA (cta_backsolve, blk_only).  Entry word:
+ * supernode | (block + 1) << 24. */
+static int bs_nblk(const plan_t *pl, int s)
+{
+    const int c = 3 * pl->desc[s].cb;
+    return !pl->bs_leaf[s] && c > 96 && pl->nsn < (1 << 24) ? (c + 95) / 96 : 1;
+}
+
+/* Writes the front_ctas(G) task entries of front s (workers 0 .. G-1 of a team, consecutive); returns their number. */
+static int emit_front(int *tasks, int *nwait, int s, int nw, int G)
+{
+    const int n = front_ctas(G);
+    for (int w = 0; w < n; w++) {
+        tasks[w] = s;
+        nwait[w] = pack_nwait(nw, w, G);
+    }
+    return n;
+}
+
+/* The task lists of this rank: leaf_tasks (k_factor_leaf), tasks/nwait (k_factor: own fronts outside the leaf set)
+ * and top_tasks/top_nwait (k_factor: the fronts above a multi-GPU cut), each in the ticket order `tick`; btasks =
+ * [top | own shards outside the back-solve leaf set | that set], each segment in the back-solve order `bso`. */
+static void emit_lists(plan_t *pl, const int *owner, int me, const char *leaf, const int *G, const int *tick,
+                       const int *bso)
+{
+    const int nsn = pl->nsn;
+    free(pl->tasks); free(pl->nwait); free(pl->btasks); free(pl->leaf_tasks); free(pl->top_tasks); free(pl->top_nwait);
+    int n_local = 0, n_top = 0, n_leaf = 0, n_top_sn = 0, n_main_bt = 0, n_top_bt = 0;
     for (int s = 0; s < nsn; s++) {
         if (owner[s] == me) {
             if (leaf[s])
                 n_leaf++;
             else
-                n_local += G_of[s] < 0 ? 1 : G_of[s];
+                n_local += front_ctas(G[s]);
             if (!pl->bs_leaf[s])
-                n_main_sn += BS_NBLK(s);
+                n_main_bt += bs_nblk(pl, s);
         } else if (owner[s] == -1) {
-            n_top += G_of[s] < 0 ? 1 : G_of[s];
+            n_top += front_ctas(G[s]);
             n_top_sn++;
-            n_top_bt += BS_NBLK(s);
+            n_top_bt += bs_nblk(pl, s);
         }
     }
-    pl->ntasks = (int) n_local;
+    pl->ntasks = n_local;
     pl->tasks = malloc(sizeof(int) * (size_t) (n_local + 1));
     pl->nwait = malloc(sizeof(int) * (size_t) (n_local + 1));
     pl->n_leaf = n_leaf;
     pl->leaf_tasks = malloc(sizeof(int) * (size_t) (n_leaf + 1));
-    pl->n_top = (int) n_top;
+    pl->n_top = n_top;
     pl->n_top_sn = n_top_sn;
     pl->top_tasks = malloc(sizeof(int) * (size_t) (n_top + 1));
     pl->top_nwait = malloc(sizeof(int) * (size_t) (n_top + 1));
-    pl->n_bs_leaf = n_bsl;
-    pl->n_btasks = n_top_bt + n_main_sn + n_bsl;
+    pl->n_btasks = n_top_bt + n_main_bt + pl->n_bs_leaf;
     pl->btasks = malloc(sizeof(int) * (size_t) (pl->n_btasks + 1));
-    /* back-solve list, parents first: [top | own shards outside the back-solve leaf set | that set].
-     * Order inside a segment: by the modelled TIME of the longest chain below a supernode (its own solve included),
-     * longest first -- a parent's chain is longer than any child's, so the order is topological, and the deep
-     * chains do not queue behind the thousands of supernodes that merely share their height (level order: the
-     * bottom of the longest chain of the 100 k world got its tickets late at every link).  ASAM_BS_ORDER=level
-     * keeps the height order (A/B). */
-    {
-        const char *eb = getenv("ASAM_BS_ORDER");
-        if (!(eb && strcmp(eb, "level") == 0) && nsn > 0) {
-            double *down = calloc((size_t) nsn, sizeof(double));
-            sn_key_t *keys = malloc(sizeof(sn_key_t) * (size_t) nsn);
-            for (int s = 0; s < nsn; s++) { /* children have smaller ids: down[s] holds max over children here */
-                if (!pl->bs_leaf[s]) /* (the warp-per-supernode set runs in a launch of its own, afterwards) */
-                    down[s] += 5.0 + 0.17 * 3.0 * pl->desc[s].cb + 0.01 * 3.0 * pl->desc[s].mb;
-                else
-                    down[s] += 1e-3 * (pl->desc[s].level + 1);
-                const int par = pl->desc[s].parent;
-                if (par >= 0 && down[s] > down[par])
-                    down[par] = down[s];
-                keys[s].key = down[s];
-                keys[s].id = s;
-            }
-            qsort(keys, (size_t) nsn, sizeof(sn_key_t), cmp_key_desc);
-            for (int k = 0; k < nsn; k++)
-                bylv[nsn - 1 - k] = keys[k].id; /* ascending: the list below is filled backwards */
-            free(keys);
-            free(down);
-        }
+    pl->bt_split = 0;
+    int at[3] = { 0, n_top_bt, n_top_bt + n_main_bt }; /* next entry of each back-solve segment */
+    for (int k = 0; k < nsn; k++) {
+        const int s = bso[k];
+        if (owner[s] != me && owner[s] != -1)
+            continue;
+        const int seg = owner[s] == -1 ? 0 : pl->bs_leaf[s] ? 2 : 1, nb = bs_nblk(pl, s);
+        for (int b = nb - 1; b >= 0; b--) /* the last block first */
+            pl->btasks[at[seg]++] = nb > 1 ? (s | ((b + 1) << 24)) : s;
+        pl->bt_split |= nb > 1;
     }
     int t = 0, tl = 0, tt = 0;
-    int bt = n_top_bt - 1, bm = n_top_bt + n_main_sn - 1, bl = pl->n_btasks - 1;
-    for (int k = 0; k < nsn; k++) { /* back-solve entries, filled backwards: parents first */
-        int s = bylv[k];
-        if (owner[s] == -1) {
-            const int nb = BS_NBLK(s); /* block 0 lands last, the last block first */
-            for (int b = 0; b < nb; b++)
-                pl->btasks[bt--] = nb > 1 ? (s | ((b + 1) << 24)) : s;
-            pl->bt_split |= nb > 1;
-        } else if (owner[s] == me) {
-            if (pl->bs_leaf[s]) {
-                pl->btasks[bl--] = s;
-            } else {
-                const int nb = BS_NBLK(s);
-                for (int b = 0; b < nb; b++)
-                    pl->btasks[bm--] = nb > 1 ? (s | ((b + 1) << 24)) : s;
-                pl->bt_split |= nb > 1;
-            }
-        }
-    }
-    for (int k = 0; k < nsn; k++) { /* factorisation tasks, children first */
-        int s = byl[k];
+    for (int k = 0; k < nsn; k++) {
+        const int s = tick[k];
         if (owner[s] == -1) {
             int nw = 0; /* children above the cut: the others were exchanged before this launch */
             for (int c = 0; c < pl->snh[s].children.n; c++)
                 nw += owner[pl->snh[s].children.p[c]] == -1;
-            int G = G_of[s] < 0 ? 1 : G_of[s];
-            for (int w = 0; w < G; w++, tt++) {
-                pl->top_tasks[tt] = s;
-                pl->top_nwait[tt] = pack_nwait(nw, w, G > 1 ? G : (G_of[s] < 0 ? 1 : 0));
-            }
-            continue;
-        }
-        if (owner[s] != me)
-            continue;
-        if (leaf[s]) {
+            tt += emit_front(pl->top_tasks + tt, pl->top_nwait + tt, s, nw, G[s]);
+        } else if (owner[s] == me && leaf[s]) {
             pl->leaf_tasks[tl++] = s;
-            continue;
-        }
-        /* nwait counts ALL children: those of the leaf set arrived in the earlier launch */
-        int G = G_of[s] < 0 ? 1 : G_of[s];
-        for (int w = 0; w < G; w++, t++) {
-            pl->tasks[t] = s;
-            pl->nwait[t] = pack_nwait(pl->desc[s].ch_cnt, w, G > 1 ? G : (G_of[s] < 0 ? 1 : 0));
+        } else if (owner[s] == me) { /* nwait counts ALL children: those of the leaf set arrived in the earlier launch */
+            t += emit_front(pl->tasks + t, pl->nwait + t, s, pl->desc[s].ch_cnt, G[s]);
         }
     }
-#undef BS_NBLK
-    free(G_of);
-    free(byl);
-    free(bylv);
+}
+
+static void build_schedule(plan_t *pl)
+{
+    const int me = pl->world > 1 ? pl->rank : 0;
+    int *owner = shard_cut(pl, pl->world > 1 ? pl->world : 1);
+    char *leaf = leaf_sets(pl, owner, me);
+    int *G = team_sizes(pl, owner, me, leaf);
+    int *tick = factor_order(pl, owner, me, leaf, G);
+    int *bso = backsolve_order(pl);
+    emit_lists(pl, owner, me, leaf, G, tick, bso);
+    free(bso);
+    free(tick);
+    free(G);
     free(leaf);
     free(owner);
 }
@@ -1874,18 +1861,16 @@ int plan_append(plan_t *pl, asam_dev_t *dev, int N, int n_factors, const int *ft
             /* expand big fronts into teams of consecutive entries */
             int total = 0;
             for (int t = 0; t < nt; t++)
-                total += team_size(pl->desc[tasks[t]].mb, pl->desc[tasks[t]].cb, plan_team_cap(pl));
+                total += front_ctas(team_size(pl->desc[tasks[t]].mb, pl->desc[tasks[t]].cb, plan_team_cap(pl)));
             if (total != nt) {
                 int *t2 = malloc(sizeof(int) * (size_t) total), *w2 = malloc(sizeof(int) * (size_t) total);
                 int *k2 = calloc((size_t) total, sizeof(int)); /* teams re-factor whole fronts */
                 int k = 0;
                 for (int t = 0; t < nt; t++) {
-                    int G = team_size(pl->desc[tasks[t]].mb, pl->desc[tasks[t]].cb, plan_team_cap(pl));
-                    for (int w = 0; w < G; w++, k++) {
-                        t2[k] = tasks[t];
-                        w2[k] = pack_nwait(nwait[t], w, G > 1 ? G : 0);
-                        k2[k] = G > 1 ? 0 : keep[t];
-                    }
+                    const int G = team_size(pl->desc[tasks[t]].mb, pl->desc[tasks[t]].cb, plan_team_cap(pl));
+                    if (G == 0)
+                        k2[k] = keep[t];
+                    k += emit_front(t2 + k, w2 + k, tasks[t], nwait[t], G);
                 }
                 free(tasks);
                 free(nwait);

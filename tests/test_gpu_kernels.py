@@ -531,9 +531,7 @@ SWITCHES = {
     "solo400_pb12": {"ASAM_SOLO_MAX_M": "400", "ASAM_SOLO_PB": "12"}, "tpw2": {"ASAM_TILES_PER_WORKER": "2"},
     "merge_pct0": {"ASAM_TEAM_MERGE_PCT": "0"}, "plan_threads1": {"ASAM_PLAN_THREADS": "1"},
     "bs_threads128": {"ASAM_BS_THREADS": "128"},
-    "order_level": {"ASAM_TASK_ORDER": "level"}, "order_cp": {"ASAM_TASK_ORDER": "cp"},
-    "order_sim": {"ASAM_TASK_ORDER": "sim"}, "bs_order_level": {"ASAM_BS_ORDER": "level"},
-    "bs_split0": {"ASAM_BS_SPLIT": "0"},
+    "order_cp": {"ASAM_TASK_ORDER": "cp"}, "order_sim": {"ASAM_TASK_ORDER": "sim"},
 }
 REPLAY_SWITCHES = {"keep0": {"ASAM_KEEP": "0"}, "small_step0": {"ASAM_SMALL_STEP": "0"}}
 

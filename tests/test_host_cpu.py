@@ -375,6 +375,76 @@ def test_sharded_schedule_emulated(world):
     assert np.abs(st - ref).max() < 1e-9 * max(1.0, np.abs(ref).max())
 
 
+def check_factor_list(tasks, nwait, parent, nw_want):
+    """One k_factor list: every front is one run of max(G, 1) entries (workers 0 .. G-1, the same G), after the runs
+    of its children in the list; the child count of every entry is nw_want[s].  Returns {supernode: G}."""
+    G = (nwait >> 24) & 0x7F
+    first, k = {}, 0
+    while k < len(tasks):
+        s, g = int(tasks[k]), int(G[k])
+        n = max(g, 1)
+        assert s not in first and (tasks[k:k + n] == s).all() and (G[k:k + n] == g).all(), (s, k)
+        assert list((nwait[k:k + n] >> 16) & 0xFF) == list(range(n)), (s, k)
+        assert ((nwait[k:k + n] & 0xFFFF) == nw_want[s]).all(), (s, nwait[k] & 0xFFFF, nw_want[s])
+        first[s] = k
+        k += n
+    assert all(first[int(parent[s])] > k for s, k in first.items() if int(parent[s]) in first), "children first"
+    return {s: int(G[k]) for s, k in first.items()}
+
+
+SCHEDULE_ENVS = {"auto": {}, "cp": {"ASAM_TASK_ORDER": "cp"}, "sim": {"ASAM_TASK_ORDER": "sim"},
+                 "room1_min1": {"ASAM_TEAM_ROOM": "1", "ASAM_TEAM_MIN": "1"},
+                 "room1_min2": {"ASAM_TEAM_ROOM": "1", "ASAM_TEAM_MIN": "2"}}
+
+
+@pytest.mark.parametrize("env", list(SCHEDULE_ENVS))
+@pytest.mark.parametrize("n,world,auto", [(4000, 1, "cp"), (30000, 1, "sim"), (6000, 3, "cp"), (30000, 3, None)])
+def test_schedule_task_lists(monkeypatch, n, world, auto, env):
+    """The lists of a batch schedule under either ticket order and any team sizes: k_factor's main and top lists
+    (children first, teams as consecutive entries, child counts), and the batch back-solve list (one entry per
+    96-column block of the wide supernodes outside the back-solve leaf set, last block first; no other split)."""
+    d = datasets.manhattan_dense(n, seed=1)
+    ftype, fa, fb, _, _ = factor_arrays(d)
+    for k, v in SCHEDULE_ENVS[env].items():
+        monkeypatch.setenv(k, v)
+    plans = [HostPlan().build(d.n_nodes, ftype, fa, fb, world=world, rank=r) for r in range(world)]
+    if env == "auto" and auto:  # the automatic choice of this world, so that both branches are checked
+        monkeypatch.setenv("ASAM_TASK_ORDER", auto)
+        forced = HostPlan().build(d.n_nodes, ftype, fa, fb, world=world, rank=0)
+        assert np.array_equal(forced.array("tasks"), plans[0].array("tasks"))
+    D = plans[0].descs()
+    parent, cb = D["parent"], D["cb"]
+    top = set(int(s) for s in plans[0].array("top_tasks"))
+    top_children = np.zeros(len(parent) + 1, np.int64)
+    for s in top:
+        if parent[s] >= 0:
+            top_children[parent[s]] += 1
+    words = {}
+    for p in plans:
+        words.update(check_factor_list(p.array("tasks"), p.array("nwait"), parent, D["ch_cnt"]))
+        words.update(check_factor_list(p.array("top_tasks"), p.array("top_nwait"), parent, top_children))
+        bt = p.array("btasks")
+        sn, blk = bt & 0xFFFFFF, bt >> 24
+        n_bsl = p.info()["n_bs_leaf"]
+        assert (blk[len(bt) - n_bsl:] == 0).all()
+        k = 0
+        while k < len(bt):
+            s = int(sn[k])
+            nb = (3 * int(cb[s]) + 95) // 96 if 3 * cb[s] > 96 and k < len(bt) - n_bsl else 1
+            want = list(range(nb, 0, -1)) if nb > 1 else [0]
+            assert list(blk[k:k + nb]) == want and (sn[k:k + nb] == s).all(), (s, list(blk[k:k + nb]), want)
+            k += nb
+        assert len(set(int(s) for s in sn)) == len([k for k in range(len(bt)) if blk[k] <= 1]), "one run per supernode"
+    G = np.array(list(words.values()))
+    assert (G != 1).all() or env == "room1_min1", "a team of one only where ASAM_TEAM_MIN=1 asks for it"
+    if n >= 30000:  # worlds with team fronts
+        assert (G >= 2).any() or env == "room1_min1"
+        if env == "room1_min1":
+            assert (G == 1).any()
+        if env == "room1_min2":
+            assert set(G[G > 0]) == {2}
+
+
 @pytest.mark.parametrize("n0,n1,step", [(1, 40, 1), (120, 200, 1), (300, 330, 3)])
 def test_emulated_incremental_append(m3500, n0, n1, step):
     """plan_append: re-factoring only the marked supernodes reproduces the full solution."""
