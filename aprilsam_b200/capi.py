@@ -62,6 +62,10 @@ def lib() -> C.CDLL:
     L.asam_dbg_profile.restype = None
     L.asam_upload_loss.argtypes = [C.c_void_p, C.c_int, C.c_int, _ip, _dp]
     L.asam_debug_read_buffer.argtypes = [C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_void_p]
+    L.asam_marginal_cov.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, _dp]
+    L.asam_dbg_plan_marginal_paths.argtypes = [C.c_void_p, C.c_int, _ip, C.c_void_p, C.POINTER(C.c_int64)]
+    L.aprilsam_b200_marginal_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_int, _ip, _dp]
+    L.aprilsam_b200_relative_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, _dp]
     L.asam_dbg_factor_loss.argtypes = [C.c_void_p, C.c_int, _ip, _dp]
     L.asam_chi2.argtypes = [C.c_void_p, C.c_int, _dp]
     _lib = L

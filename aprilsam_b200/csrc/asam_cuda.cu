@@ -145,6 +145,8 @@ struct asam_dev {
     int trace_nfac = 0, trace_nbs = 0;
     Buf ptrace; // panel-step stamps of one team front (asam_set_panel_trace)
     int ptrace_sn = -1, ptrace_panels = 0;
+    Buf marg;          // scratch of asam_marginal_cov, allocated at the first query
+    int marg_smem = 0; // dynamic shared memory k_marginal_path is set up for
 };
 
 static int flush_uploads(asam_dev *d);
@@ -623,7 +625,7 @@ ASAM_EXPORT void asam_dev_destroy(asam_dev_t *d)
     Buf *all[] = { &d->f_type, &d->f_a, &d->f_b, &d->f_z, &d->f_W, &d->f_slot, &d->f_loss, &d->lp, &d->st, &d->node2q, &d->q2node,
                    &d->Adiag, &d->Aoff, &d->Bq, &d->y, &d->x, &d->dinv, &d->sn, &d->ipool, &d->arena, &d->arrive,
                    &d->xdone, &d->xblk, &d->tbar, &d->tasks_full, &d->nwait_full, &d->btasks_full, &d->tasks_tmp, &d->nwait_tmp,
-                   &d->btasks_tmp, &d->keep_tmp, &d->leaf_tasks, &d->top_tasks, &d->top_nwait, &d->ctrl, &d->partial, &d->patch_ids, &d->patch_desc, &d->pts, &d->flush, &d->trace_fac, &d->trace_bs, &d->ptrace };
+                   &d->btasks_tmp, &d->keep_tmp, &d->leaf_tasks, &d->top_tasks, &d->top_nwait, &d->ctrl, &d->partial, &d->patch_ids, &d->patch_desc, &d->pts, &d->flush, &d->trace_fac, &d->trace_bs, &d->ptrace, &d->marg };
     for (int i = 0; i < 2; i++)
         if (d->tev[i])
             cudaEventDestroy(d->tev[i]);
@@ -1373,6 +1375,68 @@ ASAM_EXPORT int asam_chi2(asam_dev_t *d, int n_factors, double *chi2_out)
     d->n_launch += 2;
     CK(cudaGetLastError());
     return download(d, chi2_out, partial, sizeof(double));
+}
+
+static size_t align256(size_t v) { return (v + 255) & ~(size_t) 255; }
+
+ASAM_EXPORT int asam_marginal_cov(asam_dev_t *d, int n, const asam_marg_path_t *paths, int64_t z_doubles, int n_hops,
+                                  int max_m, double *out)
+{
+    if (n < 1 || n > 65535 || !paths || !out || z_doubles < 3 || n_hops < n || max_m < 3)
+        return set_err("asam_marginal_cov: invalid arguments (n %d, z %lld, hops %d, max_m %d)", n, (long long) z_doubles,
+                       n_hops, max_m);
+    CK(cudaSetDevice(d->device));
+    const size_t smem = ASAM_MSMEM(max_m) * sizeof(double);
+    if ((int) smem > d->marg_smem) {
+        int optin = 0;
+        CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, d->device));
+        if (smem > (size_t) optin)
+            return set_err("asam_marginal_cov: fronts of order %d need %zu KB of shared memory, the device offers %d KB",
+                           max_m, smem / 1024, optin / 1024);
+        CK(cudaFuncSetAttribute(k_marginal_path, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
+        d->marg_smem = (int) smem;
+    }
+    // scratch: [err | out (3n x 3n)] [paths] [z] [hops]; err and out come back with one copy
+    const size_t out_bytes = 16 + 9 * (size_t) n * n * sizeof(double);
+    const size_t o_paths = align256(out_bytes);
+    const size_t o_z = o_paths + align256((size_t) n * sizeof(asam_marg_path_t));
+    const size_t o_hop = o_z + align256((size_t) z_doubles * sizeof(double));
+    const size_t total = o_hop + align256(4 * (size_t) n_hops * sizeof(int));
+    if (buf_reserve(d, d->marg, total, false, false))
+        return 1;
+    char *base = (char *) d->marg.p;
+    if (flush_uploads(d))
+        return 1;
+    CK(cudaMemcpyAsync(base + o_paths, paths, (size_t) n * sizeof(asam_marg_path_t), cudaMemcpyHostToDevice, d->stream));
+    CK(cudaMemsetAsync(base, 0, 16, d->stream));
+    d->n_h2d += (int64_t) n * (int64_t) sizeof(asam_marg_path_t);
+    MargArgs a;
+    a.sn = (const asam_sn_desc_t *) d->sn.p;
+    a.ipool = (const int *) d->ipool.p;
+    a.arena = (const double *) d->arena.p;
+    a.dinv = (const double *) d->dinv.p;
+    a.paths = (const asam_marg_path_t *) (base + o_paths);
+    a.z = (double *) (base + o_z);
+    a.hop = (int *) (base + o_hop);
+    a.out = (double *) (base + 16);
+    a.err = (int *) base;
+    a.n = n;
+    a.max_m = max_m;
+    k_marginal_path<<<n, 256, smem, d->stream>>>(a);
+    CK(cudaGetLastError());
+    k_marginal_gram<<<dim3(n, n), 128, 0, d->stream>>>(a);
+    CK(cudaGetLastError());
+    d->n_launch += 2;
+    std::vector<double> host(out_bytes / sizeof(double));
+    if (download(d, host.data(), base, out_bytes))
+        return 1;
+    int err = 0;
+    memcpy(&err, host.data(), sizeof(int));
+    if (err)
+        return set_err("asam_marginal_cov: %s", err == 1 ? "a front on a path is larger than max_m"
+                                                          : "a path's length differs from the plan's");
+    memcpy(out, host.data() + 2, 9 * (size_t) n * n * sizeof(double));
+    return 0;
 }
 
 // A non-zero status is fatal for the solve in flight; the control words (tickets, team barriers,

@@ -2593,3 +2593,248 @@ __global__ void k_clear_range(double *Adiag, double *Bq, double *Aoff, int q_fir
     else if (i < nd + nb + no)
         Aoff[9 * (size_t) s_first + (i - nd - nb)] = 0.0;
 }
+
+// ------------------------------------------------------------------------------------------
+// marginal covariances: Sigma = A^-1 = P' L^-T L^-1 P from the factor the last solve left in the arena
+// ------------------------------------------------------------------------------------------
+// Z_i = L^-1 E_q (three columns) is non-zero only on the supernodes from the pose's own up to the root, and
+// the path is a chain: every supernode on it gets its right-hand side from exactly one child.  Neither kernel
+// writes anything the solve path reads (arena, x, y, dinv, Hessian, control words): only the scratch below.
+struct MargArgs {
+    const asam_sn_desc_t *sn;
+    const int *ipool;
+    const double *arena;
+    const double *dinv;
+    const asam_marg_path_t *paths;
+    double *z;   // per pose: 3 doubles per scalar row of its path (row-major: row, column of E_q)
+    int *hop;    // per hop: supernode, first row js, c, offset of its rows from the pose's zoff
+    double *out; // (3n x 3n) row-major
+    int *err;    // 0 ok, 1 front larger than max_m, 2 path length differs from the plan's
+    int n, max_m;
+};
+
+#define ASAM_MLS (ASAM_BSW + 1) // leading dimension of the staged L11 block (odd: no bank conflicts)
+#define ASAM_MKG 24             // columns of a block per thread group of the trailing update (4 groups x 24 = ASAM_BSW)
+#define ASAM_MROWS 128          // rows of the trailing update per pass (2 per thread of a group)
+#define ASAM_MSMEM(max_m) (6 * (size_t) (max_m) + ASAM_BSW * ASAM_MLS + ASAM_BSW + 4 * ASAM_MROWS * 3) // doubles
+
+// One CTA per requested pose.  At each supernode s of its path (m rows, c own columns), with b the m x 3
+// right-hand side: L11 z = b[js, c) block by block (ASAM_BSW columns, the diagonal block staged in shared
+// memory and solved by one warp with the pivots 1/L_kk from dinv, as cta_backsolve uses them), after each block
+// b[be, m) -= L[be:m, block] z_block by all threads (24 loads of L in flight per row and thread: the path is a
+// dependent chain, latency is what counts).  Then z_s goes to the scratch and u = b[c, m) to the parent's rows
+// through rel.
+__global__ void __launch_bounds__(256) k_marginal_path(MargArgs a)
+{
+    extern __shared__ __align__(16) double sm[];
+    const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5, nwarps = nt >> 5;
+    const asam_marg_path_t P = a.paths[blockIdx.x];
+    double *b = sm, *bn = sm + 3 * (size_t) a.max_m;
+    double *Ls = bn + 3 * (size_t) a.max_m;
+    double *rd = Ls + ASAM_BSW * ASAM_MLS;
+    double *part = rd + ASAM_BSW; // [4 groups][ASAM_MROWS rows][3]
+    int s = P.sn0, js = P.j0, h = 0;
+    int64_t zo = P.zoff;
+    asam_sn_desc_t d = a.sn[s];
+    int m = 3 * d.mb;
+    if (m > a.max_m) {
+        if (tid == 0)
+            atomicCAS(a.err, 0, 1);
+        return;
+    }
+    for (int i = tid; i < 3 * m; i += nt)
+        b[i] = 0.0;
+    __syncthreads();
+    if (tid < 3)
+        b[3 * (js + tid) + tid] = 1.0;
+    __syncthreads();
+    for (;;) {
+        const int c = 3 * d.cb, ld = ASAM_LD(m);
+        const double *Lg = a.arena + d.f_off;
+        for (int b0 = js; b0 < c; b0 += ASAM_BSW) {
+            const int bw = min(ASAM_BSW, c - b0), be = b0 + bw;
+            for (int k = warp; k < bw; k += nwarps)
+                for (int j = k + lane; j < bw; j += 32)
+                    Ls[j + k * ASAM_MLS] = Lg[(b0 + j) + (size_t) (b0 + k) * ld];
+            for (int k = tid; k < bw; k += nt)
+                rd[k] = a.dinv[3 * (size_t) d.first + b0 + k];
+            __syncthreads();
+            // L11 z = b, left to right: z_k = b_k / L_kk, then b_j -= L[j, k] z_k for j > k.  Lane l holds rows
+            // l, l+32, l+64 of the block, z_k travels by shuffle.
+            if (warp == 0) {
+                double w[3][3];
+#pragma unroll
+                for (int t3 = 0; t3 < 3; t3++)
+#pragma unroll
+                    for (int e = 0; e < 3; e++)
+                        w[t3][e] = lane + 32 * t3 < bw ? b[3 * (b0 + lane + 32 * t3) + e] : 0.0;
+                for (int k = 0; k < bw; ++k) {
+                    const int ks = k >> 5;
+                    double zk[3];
+#pragma unroll
+                    for (int e = 0; e < 3; e++) {
+                        const double mine = ks == 0 ? w[0][e] : (ks == 1 ? w[1][e] : w[2][e]);
+                        zk[e] = __shfl_sync(0xffffffffu, mine, k & 31) * rd[k];
+                    }
+#pragma unroll
+                    for (int t3 = 0; t3 < 3; t3++) {
+                        const int j = lane + 32 * t3;
+                        if (j > k && j < bw) {
+                            const double l = Ls[j + k * ASAM_MLS];
+#pragma unroll
+                            for (int e = 0; e < 3; e++)
+                                w[t3][e] -= l * zk[e];
+                        } else if (j == k) {
+#pragma unroll
+                            for (int e = 0; e < 3; e++)
+                                w[t3][e] = zk[e];
+                        }
+                    }
+                }
+#pragma unroll
+                for (int t3 = 0; t3 < 3; t3++)
+                    if (lane + 32 * t3 < bw)
+#pragma unroll
+                        for (int e = 0; e < 3; e++)
+                            b[3 * (b0 + lane + 32 * t3) + e] = w[t3][e];
+            }
+            __syncthreads();
+            // b[be, m) -= L[be:m, b0:be] z: thread = (row slot rs, column group kg), two rows per pass; the four
+            // groups' partial sums are added in a fixed order
+            const int rs = tid & 63, kg = tid >> 6, k0 = kg * ASAM_MKG, k1 = min(k0 + ASAM_MKG, bw);
+            for (int base = be; base < m; base += ASAM_MROWS) {
+                const int i0 = base + rs, i1 = i0 + 64;
+                double a0[3] = {0.0, 0.0, 0.0}, a1[3] = {0.0, 0.0, 0.0};
+                if (k0 < k1) {
+                    double l0[ASAM_MKG], l1[ASAM_MKG];
+#pragma unroll
+                    for (int u = 0; u < ASAM_MKG; u++) {
+                        const size_t col = (size_t) (b0 + k0 + u) * ld;
+                        l0[u] = (k0 + u < k1 && i0 < m) ? Lg[i0 + col] : 0.0;
+                        l1[u] = (k0 + u < k1 && i1 < m) ? Lg[i1 + col] : 0.0;
+                    }
+#pragma unroll
+                    for (int u = 0; u < ASAM_MKG; u++) {
+                        if (k0 + u < k1) {
+                            const double *zk = b + 3 * (b0 + k0 + u);
+#pragma unroll
+                            for (int e = 0; e < 3; e++) {
+                                a0[e] += l0[u] * zk[e];
+                                a1[e] += l1[u] * zk[e];
+                            }
+                        }
+                    }
+                }
+#pragma unroll
+                for (int e = 0; e < 3; e++) {
+                    part[(kg * ASAM_MROWS + rs) * 3 + e] = a0[e];
+                    part[(kg * ASAM_MROWS + rs + 64) * 3 + e] = a1[e];
+                }
+                __syncthreads();
+                for (int q = tid; q < 3 * ASAM_MROWS; q += nt) {
+                    const int r = q / 3, e = q % 3, i = base + r;
+                    if (i < m)
+                        b[3 * i + e] -= ((part[r * 3 + e] + part[(ASAM_MROWS + r) * 3 + e]) +
+                                         part[(2 * ASAM_MROWS + r) * 3 + e]) + part[(3 * ASAM_MROWS + r) * 3 + e];
+                }
+                __syncthreads();
+            }
+        }
+        for (int i = tid; i < 3 * (c - js); i += nt)
+            a.z[zo + i] = b[3 * js + i];
+        if (tid == 0 && h < P.nhop) {
+            int *hr = a.hop + 4 * ((size_t) P.hop0 + h);
+            hr[0] = s; hr[1] = js; hr[2] = c; hr[3] = (int) (zo - P.zoff);
+        }
+        zo += 3 * (c - js);
+        ++h;
+        if (d.parent < 0)
+            break;
+        // u = b[c, m) into the parent's rows
+        const int *rel = a.ipool + d.seg + d.mb;
+        const int cb = d.cb, mb = d.mb;
+        s = d.parent;
+        d = a.sn[s];
+        const int mp = 3 * d.mb;
+        if (mp > a.max_m) {
+            if (tid == 0)
+                atomicCAS(a.err, 0, 1);
+            return;
+        }
+        for (int i = tid; i < 3 * mp; i += nt)
+            bn[i] = 0.0;
+        __syncthreads();
+        for (int q = tid; q < 9 * (mb - cb); q += nt) {
+            const int row = 3 * cb + q / 3, e = q % 3;
+            bn[3 * (3 * rel[row / 3] + row % 3) + e] = b[3 * row + e];
+        }
+        __syncthreads();
+        double *t = b;
+        b = bn;
+        bn = t;
+        m = mp;
+        js = 0;
+    }
+    if (h != P.nhop && tid == 0)
+        atomicCAS(a.err, 0, 2);
+}
+
+// One CTA per pair i <= j: Sigma_ij = Z_i' Z_j over the supernodes the two paths share (a common suffix of
+// both hop lists: paths never meet again below their lowest common ancestor), from that ancestor up, each in
+// rows [max(js_i, js_j), c).  Fixed striping and a fixed reduction tree, no floating-point atomics: the block
+// depends only on the two poses.  (j, i) is written as the exact transpose.
+__global__ void __launch_bounds__(128) k_marginal_gram(MargArgs a)
+{
+    const int i = blockIdx.y, j = blockIdx.x, tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5;
+    if (i > j)
+        return;
+    __shared__ int s_ns;
+    __shared__ double red[4][9];
+    const asam_marg_path_t Pi = a.paths[i], Pj = a.paths[j];
+    const int *hi = a.hop + 4 * (size_t) Pi.hop0, *hj = a.hop + 4 * (size_t) Pj.hop0;
+    const int nmin = min(Pi.nhop, Pj.nhop);
+    if (tid == 0)
+        s_ns = nmin;
+    __syncthreads();
+    for (int t = tid; t < nmin; t += nt)
+        if (hi[4 * (Pi.nhop - 1 - t)] != hj[4 * (Pj.nhop - 1 - t)])
+            atomicMin(&s_ns, t);
+    __syncthreads();
+    double acc[9];
+#pragma unroll
+    for (int q = 0; q < 9; q++)
+        acc[q] = 0.0;
+    for (int t = s_ns - 1; t >= 0; --t) {
+        const int *ri = hi + 4 * (Pi.nhop - 1 - t), *rj = hj + 4 * (Pj.nhop - 1 - t);
+        const int c = ri[2], r0 = max(ri[1], rj[1]);
+        const double *zi = a.z + Pi.zoff + ri[3] + 3 * (r0 - ri[1]);
+        const double *zj = a.z + Pj.zoff + rj[3] + 3 * (r0 - rj[1]);
+        for (int k = tid; k < c - r0; k += nt) {
+            const double u0 = zi[3 * k], u1 = zi[3 * k + 1], u2 = zi[3 * k + 2];
+            const double v0 = zj[3 * k], v1 = zj[3 * k + 1], v2 = zj[3 * k + 2];
+            acc[0] += u0 * v0; acc[1] += u0 * v1; acc[2] += u0 * v2;
+            acc[3] += u1 * v0; acc[4] += u1 * v1; acc[5] += u1 * v2;
+            acc[6] += u2 * v0; acc[7] += u2 * v1; acc[8] += u2 * v2;
+        }
+    }
+#pragma unroll
+    for (int q = 0; q < 9; q++) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1)
+            acc[q] += __shfl_down_sync(0xffffffffu, acc[q], o);
+        if (lane == 0)
+            red[warp][q] = acc[q];
+    }
+    __syncthreads();
+    __shared__ double S[9];
+    if (tid < 9)
+        S[tid] = ((red[0][tid] + red[1][tid]) + red[2][tid]) + red[3][tid];
+    __syncthreads();
+    if (tid < 9) {
+        const int r = tid / 3, q = tid % 3;
+        const double v = (i == j && r > q) ? S[3 * q + r] : S[tid];
+        const size_t n3 = 3 * (size_t) a.n;
+        a.out[(3 * (size_t) i + r) * n3 + 3 * j + q] = v;
+        a.out[(3 * (size_t) j + q) * n3 + 3 * i + r] = v;
+    }
+}

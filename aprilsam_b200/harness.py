@@ -71,6 +71,14 @@ def _load(impl: str) -> C.CDLL:
             getattr(lib, name).argtypes = args
         elif impl == "b200":
             raise AttributeError(f"{path}: {name} missing - rebuild with aprilsam_b200.build")
+    # covariance queries: only libraries that export them (never the reference build)
+    for name, args in (("h_marginal_cov", [C.c_void_p, C.c_int, _ip, _dp]),
+                       ("h_relative_cov", [C.c_void_p, C.c_int, C.c_int, _dp])):
+        if hasattr(lib, name):
+            getattr(lib, name).argtypes = args
+            getattr(lib, name).restype = C.c_int
+    if hasattr(lib, "aprilsam_b200_last_error"):
+        lib.aprilsam_b200_last_error.restype = C.c_char_p
     lib.h_relinearize.argtypes = [C.c_void_p, C.c_int]
     lib.h_get.argtypes = [C.c_void_p, C.c_int, _dp]
     lib.h_set.argtypes = [C.c_void_p, C.c_int, _dp]
@@ -223,6 +231,22 @@ class Harness:
 
     def dof(self) -> int:
         return self.lib.h_dof(self.h)
+
+    def marginal_covariance(self, ids):
+        """aprilsam_b200_marginal_covariance: (3n x 3n) covariance of the poses `ids` from the last solve's factor.
+        Raises RuntimeError with the library's message when it returns -1."""
+        ids = np.ascontiguousarray(ids, dtype=np.int32).reshape(-1)
+        out = np.zeros((3 * len(ids), 3 * len(ids)), dtype=np.float64)
+        if self.lib.h_marginal_cov(self.h, len(ids), _i(ids), _d(out)) != 0:
+            raise RuntimeError(self.lib.aprilsam_b200_last_error().decode())
+        return out
+
+    def relative_covariance(self, a: int, b: int):
+        """aprilsam_b200_relative_covariance: 3 x 3 covariance of pose b in pose a's frame."""
+        out = np.zeros((3, 3), dtype=np.float64)
+        if self.lib.h_relative_cov(self.h, int(a), int(b), _d(out)) != 0:
+            raise RuntimeError(self.lib.aprilsam_b200_last_error().decode())
+        return out
 
     def relinearize(self, i: int):
         self.lib.h_relinearize(self.h, i)

@@ -167,10 +167,19 @@ int plan_append(plan_t *pl, asam_dev_t *dev, int N, int n_factors, const int *ft
 void plan_work(const plan_t *pl, const int *tasks, int ntasks, double *step_work, int *step_fronts, double *batch_work,
                int *batch_fronts);
 
+/* Where each pose's columns of L^-1 live during a covariance query (asam_marginal_cov): for nodes[i], its
+ * supernode sn0 and first scalar column j0 = 3 (q - first) in it, and its entries of the hop table and the
+ * scratch (one hop per supernode from sn0 to the root; 3 doubles per scalar row, from j0 in sn0 and from 0
+ * above).  A pure function of the plan.  Returns 0, or -1 (and the error text) for a node outside [0, pl->N). */
+int plan_marginal_paths(const plan_t *pl, int n, const int *nodes, asam_marg_path_t *out, int64_t *z_total,
+                        int *hop_total);
+
 /* ---- solver context (solver.c) --------------------------------------------------------- */
 void asam_graph_forget(april_graph_t *g);
 /* graph.c: loss code and k of a factor; (0, 0) for factors without a robust loss */
 void asam_factor_loss(const april_graph_factor_t *f, int32_t *loss, double *k);
+/* graph.c: Jacobians of the xyt prediction (pose b in pose a's frame) at (pa, pb), row-major 3x3 */
+void asam_xyt_jacobians(const double *pa, const double *pb, double *Ja, double *Jb);
 /* serial.c */
 extern const stype_t stype_april_graph, stype_april_graph_attr, stype_april_node_xyt, stype_april_factor_xyt,
     stype_april_factor_xytpos, stype_april_factor_xyt_robust;

@@ -19,6 +19,16 @@ ASAM_API void asam_dbg_plan_destroy(void *p)
     free(p);
 }
 
+/* plan_marginal_paths on a plan: per node 6 ints {sn0, j0, hop0, nhop, zoff (int64)}; totals[0] = doubles of
+ * scratch, totals[1] = hops */
+ASAM_API int asam_dbg_plan_marginal_paths(void *p, int n, const int *nodes, asam_marg_path_t *out, int64_t *totals)
+{
+    int hops = 0;
+    int rc = plan_marginal_paths((const plan_t *) p, n, nodes, out, &totals[0], &hops);
+    totals[1] = hops;
+    return rc;
+}
+
 ASAM_API int asam_dbg_plan_build(void *p, int N, int F, const int *ftype, const int *fa, const int *fb)
 {
     return plan_build((plan_t *) p, NULL, N, F, ftype, fa, fb);

@@ -199,6 +199,16 @@ static void eval_finish(april_graph_factor_eval_t *ev, const matd_t *W)
     ev->chi2 = ev->r[0] * X[0] + ev->r[1] * X[1] + ev->r[2] * X[2];
 }
 
+void asam_xyt_jacobians(const double *pa, const double *pb, double *Ja, double *Jb)
+{
+    double ca = cos(pa[2]), sa = sin(pa[2]);
+    double dx = pb[0] - pa[0], dy = pb[1] - pa[1];
+    const double a[9] = { -ca, -sa, -sa * dx + ca * dy, sa, -ca, -ca * dx - sa * dy, 0, 0, -1 };
+    const double b[9] = { ca, sa, 0, -sa, ca, 0, 0, 0, 1 };
+    memcpy(Ja, a, sizeof(a));
+    memcpy(Jb, b, sizeof(b));
+}
+
 static april_graph_factor_eval_t *xyt_eval_at(april_graph_factor_t *f, const double *pa, const double *pb,
                                               april_graph_factor_eval_t *ev)
 {
@@ -206,10 +216,7 @@ static april_graph_factor_eval_t *xyt_eval_at(april_graph_factor_t *f, const dou
         ev = eval_alloc(2);
     double ca = cos(pa[2]), sa = sin(pa[2]);
     double dx = pb[0] - pa[0], dy = pb[1] - pa[1];
-    double Ja[9] = { -ca, -sa, -sa * dx + ca * dy, sa, -ca, -ca * dx - sa * dy, 0, 0, -1 };
-    double Jb[9] = { ca, sa, 0, -sa, ca, 0, 0, 0, 1 };
-    memcpy(ev->jacobians[0]->data, Ja, sizeof(Ja));
-    memcpy(ev->jacobians[1]->data, Jb, sizeof(Jb));
+    asam_xyt_jacobians(pa, pb, ev->jacobians[0]->data, ev->jacobians[1]->data);
     const double *z = f->u.common.z;
     ev->r[0] = z[0] - (ca * dx + sa * dy);
     ev->r[1] = z[1] - (-sa * dx + ca * dy);

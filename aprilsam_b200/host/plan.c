@@ -1914,3 +1914,33 @@ done:
     ivec_free(&nhi);
     return rc;
 }
+
+int plan_marginal_paths(const plan_t *pl, int n, const int *nodes, asam_marg_path_t *out, int64_t *z_total,
+                        int *hop_total)
+{
+    int64_t z = 0, hops = 0;
+    for (int i = 0; i < n; i++) {
+        const int node = nodes[i];
+        if (node < 0 || node >= pl->N) {
+            asam_set_error("node %d is not in the solved graph (%d poses)", node, pl->N);
+            return -1;
+        }
+        const int q = pl->node2q[node], s0 = pl->sn_of_q[q];
+        out[i].sn0 = s0;
+        out[i].j0 = 3 * (q - pl->desc[s0].first);
+        out[i].hop0 = (int32_t) hops;
+        out[i].zoff = z;
+        int nh = 0;
+        for (int s = s0, js = out[i].j0; s >= 0; s = pl->desc[s].parent, js = 0, nh++)
+            z += 3 * (3 * (int64_t) pl->desc[s].cb - js);
+        out[i].nhop = nh;
+        hops += nh;
+        if (hops > INT32_MAX) {
+            asam_set_error("%d poses: their paths have more than 2^31 supernodes in all", n);
+            return -1;
+        }
+    }
+    *z_total = z;
+    *hop_total = (int) hops;
+    return 0;
+}

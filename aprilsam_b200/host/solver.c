@@ -1322,3 +1322,108 @@ ASAM_API int asam_dbg_last_step(april_graph_cholesky_param_t *param, int *hdr, i
     }
     return 0;
 }
+
+/* ---- marginal covariances (extension) ------------------------------------------------------------ */
+/* The solver whose factor describes g as it is now, or NULL with the reason in the error text. */
+static solver_t *marginal_solver(april_graph_t *g, april_graph_cholesky_param_t *param, const char *fn)
+{
+    if (!g || !param) {
+        asam_set_error("%s: NULL graph or param", fn);
+        return NULL;
+    }
+    solver_t *s = (solver_t *) param->chol;
+    if (!s || s->magic != SOLVER_MAGIC || !s->gc || s->gc->graph != g) {
+        asam_set_error("%s: param does not continue a solve of this graph", fn);
+        return NULL;
+    }
+    if (!s->plan_valid) {
+        asam_set_error("%s: the plan was dropped (aprilsam_b200_invalidate_plan); solve again first", fn);
+        return NULL;
+    }
+    if (zarray_size(g->nodes) != s->plan.N || zarray_size(g->factors) != s->plan.n_factors ||
+        zarray_size(g->factors) != param->factor_num) {
+        asam_set_error("%s: nodes or factors were added since the last solve (%d / %d poses, %d / %d factors)", fn,
+                       zarray_size(g->nodes), s->plan.N, zarray_size(g->factors), s->plan.n_factors);
+        return NULL;
+    }
+    if (s->plan.world > 1) {
+        asam_set_error("%s: the last batch solve was sharded over %d GPUs; a rank holds only its own shards' fronts", fn,
+                       s->plan.world);
+        return NULL;
+    }
+    return s;
+}
+
+static int marginal_run(solver_t *s, int n, const int *nodes, double *out, const char *fn)
+{
+    asam_marg_path_t *paths = malloc(sizeof(*paths) * (size_t) n);
+    int64_t z = 0;
+    int hops = 0, rc = -1;
+    if (plan_marginal_paths(&s->plan, n, nodes, paths, &z, &hops) != 0) {
+        char why[512];
+        snprintf(why, sizeof(why), "%s", g_error);
+        asam_set_error("%s: %s", fn, why);
+    } else if (asam_marginal_cov(s->gc->dev, n, paths, z, hops, s->plan.max_m, out) != 0) {
+        asam_set_error("%s: %s", fn, asam_last_error());
+    } else {
+        rc = 0;
+    }
+    free(paths);
+    return rc;
+}
+
+ASAM_API int aprilsam_b200_marginal_covariance(april_graph_t *g, april_graph_cholesky_param_t *param, int n,
+                                               const int *nodes, double *out)
+{
+    const char *fn = "aprilsam_b200_marginal_covariance";
+    if (!nodes || !out || n < 1) {
+        asam_set_error("%s: NULL nodes / out or n < 1", fn);
+        return -1;
+    }
+    solver_t *s = marginal_solver(g, param, fn);
+    return s ? marginal_run(s, n, nodes, out, fn) : -1;
+}
+
+ASAM_API int aprilsam_b200_relative_covariance(april_graph_t *g, april_graph_cholesky_param_t *param, int a, int b,
+                                               double out9[9])
+{
+    const char *fn = "aprilsam_b200_relative_covariance";
+    if (!out9) {
+        asam_set_error("%s: NULL out9", fn);
+        return -1;
+    }
+    solver_t *s = marginal_solver(g, param, fn);
+    if (!s)
+        return -1;
+    const int ids[2] = { a, b };
+    double S[36];
+    if (marginal_run(s, 2, ids, S, fn) != 0)
+        return -1;
+    /* J = [Ja Jb] of an xyt factor between a and b at the linearisation points; out = J S J' */
+    double J[18], Ja[9], Jb[9], JS[18];
+    asam_xyt_jacobians(node_at(g, a)->l_point, node_at(g, b)->l_point, Ja, Jb);
+    for (int r = 0; r < 3; r++)
+        for (int k = 0; k < 3; k++) {
+            J[6 * r + k] = Ja[3 * r + k];
+            J[6 * r + 3 + k] = Jb[3 * r + k];
+        }
+    for (int r = 0; r < 3; r++)
+        for (int c = 0; c < 6; c++) {
+            double acc = 0.0;
+            for (int k = 0; k < 6; k++)
+                acc += J[6 * r + k] * S[6 * k + c];
+            JS[6 * r + c] = acc;
+        }
+    for (int r = 0; r < 3; r++)
+        for (int c = 0; c < 3; c++) {
+            double acc = 0.0;
+            for (int k = 0; k < 6; k++)
+                acc += JS[6 * r + k] * J[6 * c + k];
+            out9[3 * r + c] = acc;
+        }
+    /* exactly symmetric, like the covariance it comes from */
+    for (int r = 0; r < 3; r++)
+        for (int c = r + 1; c < 3; c++)
+            out9[3 * c + r] = out9[3 * r + c];
+    return 0;
+}

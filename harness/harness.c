@@ -527,6 +527,19 @@ H_EXPORT void h_set_policy_ratio(hctx_t *h, double ratio)
 #endif
 }
 
+/* aprilsam_b200_marginal_covariance / _relative_covariance (extensions; absent from the reference build) */
+#ifndef HARNESS_REFERENCE
+H_EXPORT int h_marginal_cov(hctx_t *h, int n, const int *nodes, double *out)
+{
+    return aprilsam_b200_marginal_covariance(h->g, h->p, n, nodes, out);
+}
+
+H_EXPORT int h_relative_cov(hctx_t *h, int a, int b, double *out9)
+{
+    return aprilsam_b200_relative_covariance(h->g, h->p, a, b, out9);
+}
+#endif
+
 /* april_graph_cholesky_inc_solver (aprilsam.h:276): the reference never reads idxs (aprilsam.c:578-597) */
 H_EXPORT void h_inc_solver(hctx_t *h) { april_graph_cholesky_inc_solver(h->g, h->p, NULL); }
 

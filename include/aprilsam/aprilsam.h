@@ -262,6 +262,32 @@ april_graph_factor_t *aprilsam_b200_factor_xyt_robust_create(int a, int b, const
  * Like an edit of z / W: used from the next batch solve on, not by incremental steps before it. */
 int aprilsam_b200_factor_set_loss(april_graph_factor_t *f, int loss, double k);
 
+/* ---- marginal covariances (extension) ------------------------------------------------------------
+ * Uncertainty of poses from the factor L the GPU holds after the last april_graph_cholesky() or
+ * april_graph_cholesky_inc() of `graph` with `param`: Sigma = A^-1 of the system that solve factored, that is
+ * J'WJ at each factor's evaluation point (its linearisation point, not `state`) plus tikhanov on the poses
+ * that existed at the last batch solve (incremental steps give new poses no such term).  Nothing is
+ * re-factored and nothing changes: not the graph, `param`, the tree, the solver's device state or what the
+ * next call does.  The cost follows the root paths of the poses asked for.
+ *
+ * Absolute covariances of a graph without a prior are set mostly by tikhanov: about 1/tikhanov in the gauge
+ * directions.  The relative covariance is free of the gauge; it is what gating a candidate loop closure by its
+ * Mahalanobis distance needs.
+ *
+ * Both return 0, or -1 with the reason in aprilsam_b200_last_error() for NULL arguments or n < 1, node ids
+ * outside the graph, a `param` that does not continue a solve of `graph`, a plan dropped by
+ * aprilsam_b200_invalidate_plan, nodes or factors added since the last solve, or a sharded batch solve (a rank
+ * holds only its own shards' fronts).
+ *
+ * out: (3n) x (3n), row-major; block (a, b) = cov(x_nodes[a], x_nodes[b]) in (x, y, theta) order.  Exactly
+ * symmetric, the same on every call, and block (a, b) does not depend on the other nodes asked for. */
+int aprilsam_b200_marginal_covariance(april_graph_t *graph, april_graph_cholesky_param_t *param, int n, const int *nodes,
+                                      double *out);
+/* Covariance (3 x 3, row-major) of pose b expressed in pose a's frame: J Sigma_ab J' with Sigma_ab the 6 x 6 joint
+ * marginal of (a, b) and J = [J_a J_b] the Jacobians of an xyt factor between a and b at their l_points. */
+int aprilsam_b200_relative_covariance(april_graph_t *graph, april_graph_cholesky_param_t *param, int a, int b,
+                                      double out9[9]);
+
 /* Relinearisation / re-ordering policy of april_graph_cholesky_inc().  The reference escalates an
  * incremental step to a full batch solve when `start_over > nthreshold` (kept) and, as shipped, also
  * when the step took longer than a third of the last batch solve by the WALL CLOCK

@@ -171,6 +171,25 @@ int asam_download_y(asam_dev_t *d, int q_first, int q_count, double *y3);
 /* x and the factorisation status (see asam_factor_status) with a single synchronisation. */
 int asam_download_x_status(asam_dev_t *d, int q_first, int q_count, double *x3, int *status_out);
 
+/* Marginal covariances from the factor in the arena (Sigma = A^-1 = P' L^-T L^-1 P).  Pose i at elimination
+ * position q lies in supernode sn0 at scalar column j0 = 3 (q - first); its three columns Z_i = L^-1 E_q are
+ * non-zero only on the supernodes from sn0 to the root, and Sigma_ij = Z_i' Z_j sums over the supernodes the two
+ * paths share.  The host (plan_marginal_paths) gives each pose its place in the scratch: entries
+ * [hop0, hop0 + nhop) of the hop table and the doubles from zoff on, 3 per scalar row of its path (from j0 in
+ * sn0, from 0 above). */
+typedef struct asam_marg_path {
+    int32_t sn0, j0;
+    int32_t hop0, nhop;
+    int64_t zoff;
+} asam_marg_path_t;
+/* One CTA per pose walks its path (k_marginal_path), one CTA per pair i <= j sums the shared part in a fixed
+ * order (k_marginal_gram): out (3n x 3n, row-major, host memory) is exactly symmetric, the same from call to call,
+ * and block (i, j) does not depend on the other poses of the request.  max_m: the plan's largest front order
+ * (sizes shared memory).  Reads the plan, the arena and dinv; writes only its own scratch buffer, allocated at the
+ * first call.  One synchronisation. */
+int asam_marginal_cov(asam_dev_t *d, int n, const asam_marg_path_t *paths, int64_t z_doubles, int n_hops, int max_m,
+                      double *out);
+
 /* chi2 = sum 0.5 r'Wr (xyt, at state) + sum 0.5 rho(r'Wr) (robust xyt) + sum r'Wr (xytpos) over factors [0, n_factors)
  * using the st mirror (april_graph.c:79-98). Deterministic reduction. */
 int asam_chi2(asam_dev_t *d, int n_factors, double *chi2_out);
