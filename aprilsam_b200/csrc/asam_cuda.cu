@@ -15,6 +15,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <ctime>
+#include <mutex>
 #include <vector>
 
 #include "asam_cuda.h"
@@ -146,7 +147,6 @@ struct asam_dev {
     Buf ptrace; // panel-step stamps of one team front (asam_set_panel_trace)
     int ptrace_sn = -1, ptrace_panels = 0;
     Buf marg;          // scratch of asam_marginal_cov, allocated at the first query
-    int marg_smem = 0; // dynamic shared memory k_marginal_path is set up for
 };
 
 static int flush_uploads(asam_dev *d);
@@ -1379,6 +1379,48 @@ ASAM_EXPORT int asam_chi2(asam_dev_t *d, int n_factors, double *chi2_out)
 
 static size_t align256(size_t v) { return (v + 255) & ~(size_t) 255; }
 
+// Byte offsets in the query scratch: [err | out (3n x 3n)] [paths] [z] [hops]; err and out come back with one copy.
+// o = {out, paths, z, hops, total}.
+static void marg_layout(int n, int64_t z_doubles, int n_hops, size_t o[5])
+{
+    o[0] = 16;
+    o[1] = align256(o[0] + 9 * (size_t) n * n * sizeof(double));
+    o[2] = o[1] + align256((size_t) n * sizeof(asam_marg_path_t));
+    o[3] = o[2] + align256((size_t) z_doubles * sizeof(double));
+    o[4] = o[3] + align256(4 * (size_t) n_hops * sizeof(int));
+}
+
+ASAM_EXPORT void asam_debug_marginal_layout(int n, int64_t z_doubles, int n_hops, int64_t out5[5])
+{
+    size_t o[5];
+    marg_layout(n, z_doubles, n_hops, o);
+    for (int k = 0; k < 5; k++)
+        out5[k] = (int64_t) o[k];
+}
+
+// The dynamic shared memory limit of k_marginal_path is a property of the function on a device, shared by every
+// context (one per graph) in the process.  It only grows, so a launch sized at or below any value set before stays
+// valid while other threads query graphs with smaller fronts.
+static std::mutex g_marg_smem_mu;
+static std::vector<int> g_marg_smem; // per device: bytes k_marginal_path is set up for
+
+static int marg_smem_reserve(int device, size_t smem, int max_m)
+{
+    std::lock_guard<std::mutex> lock(g_marg_smem_mu);
+    if ((size_t) device >= g_marg_smem.size())
+        g_marg_smem.resize((size_t) device + 1, 0);
+    if (smem <= (size_t) g_marg_smem[device])
+        return 0;
+    int optin = 0;
+    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+    if (smem > (size_t) optin)
+        return set_err("asam_marginal_cov: fronts of order %d need %zu KB of shared memory, the device offers %d KB",
+                       max_m, smem / 1024, optin / 1024);
+    CK(cudaFuncSetAttribute(k_marginal_path, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
+    g_marg_smem[device] = (int) smem;
+    return 0;
+}
+
 ASAM_EXPORT int asam_marginal_cov(asam_dev_t *d, int n, const asam_marg_path_t *paths, int64_t z_doubles, int n_hops,
                                   int max_m, double *out)
 {
@@ -1387,21 +1429,12 @@ ASAM_EXPORT int asam_marginal_cov(asam_dev_t *d, int n, const asam_marg_path_t *
                        n_hops, max_m);
     CK(cudaSetDevice(d->device));
     const size_t smem = ASAM_MSMEM(max_m) * sizeof(double);
-    if ((int) smem > d->marg_smem) {
-        int optin = 0;
-        CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, d->device));
-        if (smem > (size_t) optin)
-            return set_err("asam_marginal_cov: fronts of order %d need %zu KB of shared memory, the device offers %d KB",
-                           max_m, smem / 1024, optin / 1024);
-        CK(cudaFuncSetAttribute(k_marginal_path, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
-        d->marg_smem = (int) smem;
-    }
-    // scratch: [err | out (3n x 3n)] [paths] [z] [hops]; err and out come back with one copy
-    const size_t out_bytes = 16 + 9 * (size_t) n * n * sizeof(double);
-    const size_t o_paths = align256(out_bytes);
-    const size_t o_z = o_paths + align256((size_t) n * sizeof(asam_marg_path_t));
-    const size_t o_hop = o_z + align256((size_t) z_doubles * sizeof(double));
-    const size_t total = o_hop + align256(4 * (size_t) n_hops * sizeof(int));
+    if (marg_smem_reserve(d->device, smem, max_m))
+        return 1;
+    size_t lay[5];
+    marg_layout(n, z_doubles, n_hops, lay);
+    const size_t out_bytes = lay[0] + 9 * (size_t) n * n * sizeof(double);
+    const size_t o_paths = lay[1], o_z = lay[2], o_hop = lay[3], total = lay[4];
     if (buf_reserve(d, d->marg, total, false, false))
         return 1;
     char *base = (char *) d->marg.p;
@@ -1499,6 +1532,8 @@ ASAM_EXPORT int asam_debug_read_buffer(asam_dev_t *d, int id, int64_t off, int64
     case ASAM_DBG_BUF_FZ: b = &d->f_z; break;
     case ASAM_DBG_BUF_FW: b = &d->f_W; break;
     case ASAM_DBG_BUF_FLOSS: b = &d->f_loss; break;
+    case ASAM_DBG_BUF_DINV: b = &d->dinv; break;
+    case ASAM_DBG_BUF_MARG: b = &d->marg; break;
     default: return set_err("asam_debug_read_buffer: unknown buffer id %d", id);
     }
     if (off < 0 || bytes < 0 || (size_t) (off + bytes) > b->cap)

@@ -207,12 +207,17 @@ int asam_factor_status(asam_dev_t *d, int *status_out);
 int asam_debug_read_hessian(asam_dev_t *d, int n_nodes, int n_slots, double *Adiag9, double *Aoff9, double *Bq3);
 int asam_debug_read_front(asam_dev_t *d, int64_t f_off, int64_t count, double *out);
 /* bytes [off, off+bytes) of one device mirror of host state: the plan (descriptors, int pool, node2q,
- * q2node, factor slots) or the factor mirror (type, node ids, z, W, {loss, k} records) */
+ * q2node, factor slots) or the factor mirror (type, node ids, z, W, {loss, k} records); the reciprocal pivots
+ * 1/L_kk (dinv, 3 doubles per pose in elimination order) or the scratch of the last asam_marginal_cov */
 enum {
     ASAM_DBG_BUF_SN = 0, ASAM_DBG_BUF_IPOOL, ASAM_DBG_BUF_NODE2Q, ASAM_DBG_BUF_Q2NODE, ASAM_DBG_BUF_FSLOT,
-    ASAM_DBG_BUF_FTYPE, ASAM_DBG_BUF_FA, ASAM_DBG_BUF_FB, ASAM_DBG_BUF_FZ, ASAM_DBG_BUF_FW, ASAM_DBG_BUF_FLOSS
+    ASAM_DBG_BUF_FTYPE, ASAM_DBG_BUF_FA, ASAM_DBG_BUF_FB, ASAM_DBG_BUF_FZ, ASAM_DBG_BUF_FW, ASAM_DBG_BUF_FLOSS,
+    ASAM_DBG_BUF_DINV, ASAM_DBG_BUF_MARG
 };
 int asam_debug_read_buffer(asam_dev_t *d, int id, int64_t off, int64_t bytes, void *out);
+/* Byte offsets in the scratch of an asam_marginal_cov call with these arguments: {out (3n x 3n doubles), paths,
+ * z, hops (4 ints each: supernode, js, c, offset of its rows from the pose's zoff), total}; the error word is at 0. */
+void asam_debug_marginal_layout(int n, int64_t z_doubles, int n_hops, int64_t out5[5]);
 int asam_sync(asam_dev_t *d);
 /* Counters: [0] kernel launches since creation, [1] bytes H2D, [2] bytes D2H. */
 int asam_counters(asam_dev_t *d, int64_t *out3);

@@ -283,6 +283,24 @@ def single_solve(R, h, d, fc, out, tag):
             "digests": {s: [sha(snap.fronts[s][0], snap.fronts[s][1]), paths[s]] for s in range(snap.nsn)}}
 
 
+def marginal_report(R, h, d, fc, sharded):
+    """After a sharded solve: the errors of marginal_covariance and relative_covariance (a rank holds only its own
+    shards' fronts).  After a single-GPU solve on the same context: the hop-by-hop checks of margcheck."""
+    if sharded:
+        errs = []
+        for call in (lambda: h.marginal_covariance([0, d.n_nodes - 1]), lambda: h.relative_covariance(0, 1)):
+            try:
+                call()
+                errs.append(None)
+            except RuntimeError as e:
+                errs.append(str(e))
+        return {"errors": errs}
+    from support import margcheck as mc
+    nodes = [0, d.n_nodes - 1, d.n_nodes // 2, 17]
+    _, res = mc.query_report(h, R.D, fc.snapshot(h, R.D), nodes)
+    return res
+
+
 def job_solve(R, job, fc):
     d = load_graph(job["graph"])
     out, rep = {}, {"runs": []}
@@ -296,6 +314,8 @@ def job_solve(R, job, fc):
             else:
                 R.sync()
                 r = single_solve(R, h, d, fc, out, f"run{k}")
+            if job.get("marginals"):
+                r["marginals"] = marginal_report(R, h, d, fc, on)
             rep["runs"].append(r)
     if job.get("single") and R.rank == 0:  # in a harness of its own (a fresh plan)
         R.set_sharding(0)

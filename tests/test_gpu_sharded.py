@@ -401,6 +401,21 @@ def assert_sharded(name, ranks, exact, summary):
                 cov[f"{what} rank {r} vs rank {r2}"] = [n2, len(set(dig) & set(dig2))]
 
 
+def assert_marginals(ranks):
+    """Covariance queries after each run of the sharded / one-GPU / sharded job: refused with the reason on every rank
+    after a sharded solve, checked hop by hop after the one-GPU solve on the same context."""
+    from test_gpu_marginals import DINV_C, GRAM_C, HOP_C
+    for rep, _ in ranks:
+        for run in rep["runs"]:
+            m = run["marginals"]
+            print("MARGCHECK sharded " + json.dumps(m))
+            if run["sharded"]:
+                assert all(e is not None and "sharded" in e for e in m["errors"]), m
+            else:
+                assert m["hops_bad"] == 0 and m["transpose_bad"] == 0 and m["symmetric"], m
+                assert m["hop"] <= HOP_C and m["gram"] <= GRAM_C and m["dinv"] <= DINV_C, m
+
+
 SUMMARY = {}
 
 
@@ -417,7 +432,8 @@ def test_sharded_solves(two_contexts, standin, tmp_path, world):
     jobs = []
     for k, (name, env) in enumerate(SOLVE_JOBS[world]):
         jobs.append({"name": f"{name}_{k}", "kind": "solve", "graph_name": name, "env": env, "single": True,
-                     "tikhonov": LAMBDA, "sharding": [1, 0, 1] if (name == "int30k" and world == 2) else [1]})
+                     "tikhonov": LAMBDA, "sharding": [1, 0, 1] if (name == "int30k" and world == 2) else [1],
+                     "marginals": name == "int30k" and world == 2})
     out = run_sharded(standin, tmp_path, world, jobs)
     summary = SUMMARY.setdefault(f"world{world}", {})
     for job in jobs:
@@ -425,6 +441,8 @@ def test_sharded_solves(two_contexts, standin, tmp_path, world):
         summary.setdefault("seconds", {})[job["name"]] = max(r[0]["seconds"] for r in ranks)
         assert_sharded(job["name"], ranks, True, summary)
     _report(f"world{world}")
+    if world == 2:
+        assert_marginals(out["int30k_0"])
     cov = summary["bit_identity"]
     for job in jobs:  # every job compared some fronts bit for bit with the single-GPU solve
         assert sum(n for key, (n, _) in cov.items() if key.startswith(job["name"]) and key.endswith("vs single")) > 0, cov
