@@ -66,6 +66,14 @@ def lib() -> C.CDLL:
     L.asam_dbg_plan_marginal_paths.argtypes = [C.c_void_p, C.c_int, _ip, C.c_void_p, C.POINTER(C.c_int64)]
     L.aprilsam_b200_marginal_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_int, _ip, _dp]
     L.aprilsam_b200_relative_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, _dp]
+    L.aprilsam_b200_candidate_mahalanobis.argtypes = [C.c_void_p, C.c_void_p, C.c_int, _ip, _ip, _dp, _dp, _dp, _dp]
+    L.asam_marginal_pairs.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int,
+                                      C.c_void_p, _dp]
+    L.asam_dbg_plan_candidate_batches.argtypes = [C.c_void_p, C.c_int, _ip, _ip, C.c_int64, _ip, _ip, _ip, _ip, _ip]
+    L.asam_dbg_set_candidate_budget.argtypes = [C.c_int64]
+    L.asam_dbg_set_candidate_budget.restype = None
+    L.asam_debug_marginal_pairs_layout.argtypes = [C.c_int, C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_int64)]
+    L.asam_debug_marginal_pairs_layout.restype = None
     L.asam_dbg_factor_loss.argtypes = [C.c_void_p, C.c_int, _ip, _dp]
     L.asam_chi2.argtypes = [C.c_void_p, C.c_int, _dp]
     _lib = L

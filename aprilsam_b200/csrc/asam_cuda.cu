@@ -1398,13 +1398,33 @@ ASAM_EXPORT void asam_debug_marginal_layout(int n, int64_t z_doubles, int n_hops
         out5[k] = (int64_t) o[k];
 }
 
+// Byte offsets in the scratch of a candidate query: [err | out (10 doubles per candidate)] [paths] [z] [hops] [pairs].
+// o = {out, paths, z, hops, pairs, total}.
+static void marg_pairs_layout(int n, int64_t z_doubles, int n_hops, int k, size_t o[6])
+{
+    o[0] = 16;
+    o[1] = align256(o[0] + 10 * (size_t) k * sizeof(double));
+    o[2] = o[1] + align256((size_t) n * sizeof(asam_marg_path_t));
+    o[3] = o[2] + align256((size_t) z_doubles * sizeof(double));
+    o[4] = o[3] + align256(4 * (size_t) n_hops * sizeof(int));
+    o[5] = o[4] + align256((size_t) k * sizeof(asam_marg_pair_t));
+}
+
+ASAM_EXPORT void asam_debug_marginal_pairs_layout(int n, int64_t z_doubles, int n_hops, int k, int64_t out6[6])
+{
+    size_t o[6];
+    marg_pairs_layout(n, z_doubles, n_hops, k, o);
+    for (int q = 0; q < 6; q++)
+        out6[q] = (int64_t) o[q];
+}
+
 // The dynamic shared memory limit of k_marginal_path is a property of the function on a device, shared by every
 // context (one per graph) in the process.  It only grows, so a launch sized at or below any value set before stays
 // valid while other threads query graphs with smaller fronts.
 static std::mutex g_marg_smem_mu;
 static std::vector<int> g_marg_smem; // per device: bytes k_marginal_path is set up for
 
-static int marg_smem_reserve(int device, size_t smem, int max_m)
+static int marg_smem_reserve(int device, size_t smem, int max_m, const char *fn)
 {
     std::lock_guard<std::mutex> lock(g_marg_smem_mu);
     if ((size_t) device >= g_marg_smem.size())
@@ -1414,8 +1434,8 @@ static int marg_smem_reserve(int device, size_t smem, int max_m)
     int optin = 0;
     CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
     if (smem > (size_t) optin)
-        return set_err("asam_marginal_cov: fronts of order %d need %zu KB of shared memory, the device offers %d KB",
-                       max_m, smem / 1024, optin / 1024);
+        return set_err("%s: fronts of order %d need %zu KB of shared memory, the device offers %d KB", fn, max_m,
+                       smem / 1024, optin / 1024);
     CK(cudaFuncSetAttribute(k_marginal_path, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
     g_marg_smem[device] = (int) smem;
     return 0;
@@ -1429,7 +1449,7 @@ ASAM_EXPORT int asam_marginal_cov(asam_dev_t *d, int n, const asam_marg_path_t *
                        n_hops, max_m);
     CK(cudaSetDevice(d->device));
     const size_t smem = ASAM_MSMEM(max_m) * sizeof(double);
-    if (marg_smem_reserve(d->device, smem, max_m))
+    if (marg_smem_reserve(d->device, smem, max_m, "asam_marginal_cov"))
         return 1;
     size_t lay[5];
     marg_layout(n, z_doubles, n_hops, lay);
@@ -1449,6 +1469,7 @@ ASAM_EXPORT int asam_marginal_cov(asam_dev_t *d, int n, const asam_marg_path_t *
     a.arena = (const double *) d->arena.p;
     a.dinv = (const double *) d->dinv.p;
     a.paths = (const asam_marg_path_t *) (base + o_paths);
+    a.pairs = nullptr;
     a.z = (double *) (base + o_z);
     a.hop = (int *) (base + o_hop);
     a.out = (double *) (base + 16);
@@ -1469,6 +1490,58 @@ ASAM_EXPORT int asam_marginal_cov(asam_dev_t *d, int n, const asam_marg_path_t *
         return set_err("asam_marginal_cov: %s", err == 1 ? "a front on a path is larger than max_m"
                                                           : "a path's length differs from the plan's");
     memcpy(out, host.data() + 2, 9 * (size_t) n * n * sizeof(double));
+    return 0;
+}
+
+ASAM_EXPORT int asam_marginal_pairs(asam_dev_t *d, int n, const asam_marg_path_t *paths, int64_t z_doubles,
+                                    int n_hops, int max_m, int k, const asam_marg_pair_t *pairs, double *out)
+{
+    if (n < 1 || !paths || z_doubles < 3 || n_hops < n || max_m < 3 || k < 1 || !pairs || !out)
+        return set_err("asam_marginal_pairs: invalid arguments (n %d, z %lld, hops %d, max_m %d, k %d)", n,
+                       (long long) z_doubles, n_hops, max_m, k);
+    CK(cudaSetDevice(d->device));
+    const size_t smem = ASAM_MSMEM(max_m) * sizeof(double);
+    if (marg_smem_reserve(d->device, smem, max_m, "asam_marginal_pairs"))
+        return 1;
+    size_t lay[6];
+    marg_pairs_layout(n, z_doubles, n_hops, k, lay);
+    const size_t out_bytes = lay[0] + 10 * (size_t) k * sizeof(double);
+    if (buf_reserve(d, d->marg, lay[5], false, false))
+        return 1;
+    char *base = (char *) d->marg.p;
+    if (flush_uploads(d))
+        return 1;
+    CK(cudaMemcpyAsync(base + lay[1], paths, (size_t) n * sizeof(asam_marg_path_t), cudaMemcpyHostToDevice, d->stream));
+    CK(cudaMemcpyAsync(base + lay[4], pairs, (size_t) k * sizeof(asam_marg_pair_t), cudaMemcpyHostToDevice, d->stream));
+    CK(cudaMemsetAsync(base, 0, 16, d->stream));
+    d->n_h2d += (int64_t) n * (int64_t) sizeof(asam_marg_path_t) + (int64_t) k * (int64_t) sizeof(asam_marg_pair_t);
+    MargArgs a;
+    a.sn = (const asam_sn_desc_t *) d->sn.p;
+    a.ipool = (const int *) d->ipool.p;
+    a.arena = (const double *) d->arena.p;
+    a.dinv = (const double *) d->dinv.p;
+    a.paths = (const asam_marg_path_t *) (base + lay[1]);
+    a.pairs = (const asam_marg_pair_t *) (base + lay[4]);
+    a.z = (double *) (base + lay[2]);
+    a.hop = (int *) (base + lay[3]);
+    a.out = (double *) (base + 16);
+    a.err = (int *) base;
+    a.n = n;
+    a.max_m = max_m;
+    k_marginal_path<<<n, 256, smem, d->stream>>>(a);
+    CK(cudaGetLastError());
+    k_marginal_pairs<<<k, 128, 0, d->stream>>>(a);
+    CK(cudaGetLastError());
+    d->n_launch += 2;
+    std::vector<double> host(out_bytes / sizeof(double));
+    if (download(d, host.data(), base, out_bytes))
+        return 1;
+    int err = 0;
+    memcpy(&err, host.data(), sizeof(int));
+    if (err)
+        return set_err("asam_marginal_pairs: %s", err == 1 ? "a front on a path is larger than max_m"
+                                                            : "a path's length differs from the plan's");
+    memcpy(out, host.data() + 2, 10 * (size_t) k * sizeof(double));
     return 0;
 }
 

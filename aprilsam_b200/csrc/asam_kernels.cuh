@@ -2606,9 +2606,10 @@ struct MargArgs {
     const double *arena;
     const double *dinv;
     const asam_marg_path_t *paths;
+    const asam_marg_pair_t *pairs; // k_marginal_pairs: one record per candidate
     double *z;   // per pose: 3 doubles per scalar row of its path (row-major: row, column of E_q)
     int *hop;    // per hop: supernode, first row js, c, offset of its rows from the pose's zoff
-    double *out; // (3n x 3n) row-major
+    double *out; // k_marginal_gram: (3n x 3n) row-major; k_marginal_pairs: 10 doubles per candidate
     int *err;    // 0 ok, 1 front larger than max_m, 2 path length differs from the plan's
     int n, max_m;
 };
@@ -2779,18 +2780,18 @@ __global__ void __launch_bounds__(256) k_marginal_path(MargArgs a)
         atomicCAS(a.err, 0, 2);
 }
 
-// One CTA per pair i <= j: Sigma_ij = Z_i' Z_j over the supernodes the two paths share (a common suffix of
-// both hop lists: paths never meet again below their lowest common ancestor), from that ancestor up, each in
-// rows [max(js_i, js_j), c).  Fixed striping and a fixed reduction tree, no floating-point atomics: the block
-// depends only on the two poses.  (j, i) is written as the exact transpose.
-__global__ void __launch_bounds__(128) k_marginal_gram(MargArgs a)
+// Sigma_ij = Z_i' Z_j over the supernodes the two paths share (a common suffix of both hop lists: paths never meet
+// again below their lowest common ancestor), from that ancestor up, each in rows [max(js_i, js_j), c).  Called by
+// all 128 threads of a CTA; fixed striping and a fixed reduction tree, no floating-point atomics: the block depends
+// only on the two poses.  Returns element tid (row-major) to threads tid < 9, for a diagonal block (diag) taken
+// from the upper triangle, so that the block is exactly symmetric.
+__device__ __forceinline__ double marg_block(const MargArgs &a, const asam_marg_path_t &Pi, const asam_marg_path_t &Pj,
+                                             bool diag)
 {
-    const int i = blockIdx.y, j = blockIdx.x, tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5;
-    if (i > j)
-        return;
+    const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5;
     __shared__ int s_ns;
     __shared__ double red[4][9];
-    const asam_marg_path_t Pi = a.paths[i], Pj = a.paths[j];
+    __shared__ double S[9];
     const int *hi = a.hop + 4 * (size_t) Pi.hop0, *hj = a.hop + 4 * (size_t) Pj.hop0;
     const int nmin = min(Pi.nhop, Pj.nhop);
     if (tid == 0)
@@ -2826,15 +2827,107 @@ __global__ void __launch_bounds__(128) k_marginal_gram(MargArgs a)
             red[warp][q] = acc[q];
     }
     __syncthreads();
-    __shared__ double S[9];
     if (tid < 9)
         S[tid] = ((red[0][tid] + red[1][tid]) + red[2][tid]) + red[3][tid];
     __syncthreads();
+    if (tid >= 9)
+        return 0.0;
+    const int r = tid / 3, q = tid % 3;
+    return (diag && r > q) ? S[3 * q + r] : S[tid];
+}
+
+// One CTA per pair i <= j: block (i, j) from marg_block, (j, i) written as its exact transpose.
+__global__ void __launch_bounds__(128) k_marginal_gram(MargArgs a)
+{
+    const int i = blockIdx.y, j = blockIdx.x, tid = threadIdx.x;
+    if (i > j)
+        return;
+    const double v = marg_block(a, a.paths[i], a.paths[j], i == j);
     if (tid < 9) {
         const int r = tid / 3, q = tid % 3;
-        const double v = (i == j && r > q) ? S[3 * q + r] : S[tid];
         const size_t n3 = 3 * (size_t) a.n;
         a.out[(3 * (size_t) i + r) * n3 + 3 * j + q] = v;
         a.out[(3 * (size_t) j + q) * n3 + 3 * i + r] = v;
     }
+}
+
+// One CTA per candidate factor (asam_marg_pair_t): Sigma_aa, and for a closure Sigma_ab and Sigma_bb, by marg_block
+// (each bit-identical to the block asam_marginal_cov gives), then on one thread Sigma_rel = J Sigma_6 J' in the
+// order of a row-major 3x6 by 6x6 by 6x3 product (symmetrised from its upper triangle; Sigma_aa itself for a
+// prior), S = Sigma_rel + Winv, S = L L' and d2 = |L^-1 r|^2.  A pivot of S that is not > 0 gives NaN.  The output
+// depends only on the candidate's own record: the same alone, in any request, order or batch.
+__global__ void __launch_bounds__(128) k_marginal_pairs(MargArgs a)
+{
+    const int tid = threadIdx.x;
+    const asam_marg_pair_t &pr = a.pairs[blockIdx.x];
+    const int pa = pr.pa, pb = pr.pb;
+    __shared__ double sg[3][9]; // Sigma_aa, Sigma_ab, Sigma_bb
+    const asam_marg_path_t Pa = a.paths[pa];
+    double v = marg_block(a, Pa, Pa, true);
+    if (tid < 9)
+        sg[0][tid] = v;
+    if (pb >= 0) {
+        const asam_marg_path_t Pb = a.paths[pb];
+        v = marg_block(a, Pa, Pb, false);
+        if (tid < 9)
+            sg[1][tid] = v;
+        v = marg_block(a, Pb, Pb, true);
+        if (tid < 9)
+            sg[2][tid] = v;
+    }
+    __syncthreads();
+    if (tid != 0)
+        return;
+    double R[9];
+    if (pb < 0) {
+#pragma unroll
+        for (int q = 0; q < 9; q++)
+            R[q] = sg[0][q];
+    } else {
+        // Sigma_6 = [S_aa S_ab; S_ab' S_bb], entry (k, c)
+        auto s6 = [&](int k, int c) -> double {
+            if (k < 3)
+                return c < 3 ? sg[0][3 * k + c] : sg[1][3 * k + c - 3];
+            return c < 3 ? sg[1][3 * c + k - 3] : sg[2][3 * (k - 3) + c - 3];
+        };
+        double JS[18];
+        for (int r = 0; r < 3; r++)
+            for (int c = 0; c < 6; c++) {
+                double acc = 0.0;
+                for (int k = 0; k < 6; k++)
+                    acc += pr.J[6 * r + k] * s6(k, c);
+                JS[6 * r + c] = acc;
+            }
+        for (int r = 0; r < 3; r++)
+            for (int c = r; c < 3; c++) {
+                double acc = 0.0;
+                for (int k = 0; k < 6; k++)
+                    acc += JS[6 * r + k] * pr.J[6 * c + k];
+                R[3 * r + c] = acc;
+                R[3 * c + r] = acc;
+            }
+    }
+    double *o = a.out + 10 * (size_t) blockIdx.x;
+#pragma unroll
+    for (int q = 0; q < 9; q++)
+        o[1 + q] = R[q];
+    double d2 = nan("");
+    if (pr.has_w) {
+        double S[9];
+#pragma unroll
+        for (int q = 0; q < 9; q++)
+            S[q] = R[q] + pr.Winv[q];
+        const double l00 = S[0] > 0.0 ? sqrt(S[0]) : nan("");
+        const double l10 = S[3] / l00, l20 = S[6] / l00;
+        const double e11 = S[4] - l10 * l10;
+        const double l11 = e11 > 0.0 ? sqrt(e11) : nan("");
+        const double l21 = (S[7] - l20 * l10) / l11;
+        const double e22 = (S[8] - l20 * l20) - l21 * l21;
+        const double l22 = e22 > 0.0 ? sqrt(e22) : nan("");
+        const double y0 = pr.r[0] / l00;
+        const double y1 = (pr.r[1] - l10 * y0) / l11;
+        const double y2 = ((pr.r[2] - l20 * y0) - l21 * y1) / l22;
+        d2 = (y0 * y0 + y1 * y1) + y2 * y2;
+    }
+    o[0] = d2;
 }

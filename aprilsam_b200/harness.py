@@ -73,7 +73,8 @@ def _load(impl: str) -> C.CDLL:
             raise AttributeError(f"{path}: {name} missing - rebuild with aprilsam_b200.build")
     # covariance queries: only libraries that export them (never the reference build)
     for name, args in (("h_marginal_cov", [C.c_void_p, C.c_int, _ip, _dp]),
-                       ("h_relative_cov", [C.c_void_p, C.c_int, C.c_int, _dp])):
+                       ("h_relative_cov", [C.c_void_p, C.c_int, C.c_int, _dp]),
+                       ("h_candidate_mahalanobis", [C.c_void_p, C.c_int, _ip, _ip, _dp, _dp, _dp, _dp])):
         if hasattr(lib, name):
             getattr(lib, name).argtypes = args
             getattr(lib, name).restype = C.c_int
@@ -247,6 +248,24 @@ class Harness:
         if self.lib.h_relative_cov(self.h, int(a), int(b), _d(out)) != 0:
             raise RuntimeError(self.lib.aprilsam_b200_last_error().decode())
         return out
+
+    def candidate_mahalanobis(self, a, b, z, W, with_cov: bool = False):
+        """aprilsam_b200_candidate_mahalanobis: d2 (k,) of the candidate factors (a[c], b[c]; b[c] = -1 for a prior)
+        with measurements z (k x 3) and information matrices W (k x 9 or k x 3 x 3); with_cov also returns
+        Sigma_rel (k x 3 x 3).  Raises RuntimeError with the library's message when it returns -1."""
+        a = np.ascontiguousarray(a, dtype=np.int32).reshape(-1)
+        b = np.ascontiguousarray(b, dtype=np.int32).reshape(-1)
+        k = len(a)
+        if len(b) != k:
+            raise ValueError(f"a has {k} ids, b {len(b)}")
+        z = np.ascontiguousarray(z, dtype=np.float64).reshape(k, 3)
+        W = np.ascontiguousarray(W, dtype=np.float64).reshape(k, 9)
+        d2 = np.zeros(k, dtype=np.float64)
+        cov = np.zeros((k, 3, 3), dtype=np.float64) if with_cov else None
+        if self.lib.h_candidate_mahalanobis(self.h, k, _i(a), _i(b), _d(z), _d(W), _d(d2),
+                                            _d(cov) if with_cov else None) != 0:
+            raise RuntimeError(self.lib.aprilsam_b200_last_error().decode())
+        return (d2, cov) if with_cov else d2
 
     def relinearize(self, i: int):
         self.lib.h_relinearize(self.h, i)

@@ -174,12 +174,30 @@ void plan_work(const plan_t *pl, const int *tasks, int ntasks, double *step_work
 int plan_marginal_paths(const plan_t *pl, int n, const int *nodes, asam_marg_path_t *out, int64_t *z_total,
                         int *hop_total);
 
+/* Batches of a candidate query (aprilsam_b200_candidate_mahalanobis): candidates c in input order, where candidate
+ * c is a factor on poses a[c] and b[c] (b[c] = -1: a prior on a[c]; ids valid, checked by the caller).  A batch
+ * closes before the candidate whose new poses would take the scratch of its distinct poses beyond `budget` doubles;
+ * a batch always holds at least one candidate.  Batch t holds candidates [batch_end[t-1], batch_end[t]) and the
+ * distinct poses poses[pose_end[t-1], pose_end[t]) in order of first use; ia[c] / ib[c] are the places of a[c] /
+ * b[c] in that list (ib = -1 for a prior).  poses needs room for 2k ids, batch_end and pose_end for k.  A pure
+ * function of the plan, the ids and the budget. */
+void plan_candidate_batches(const plan_t *pl, int k, const int *a, const int *b, int64_t budget, int *batch_end,
+                            int *n_batches, int *poses, int *pose_end, int *ia, int *ib);
+
+/* Bytes of z scratch a batch of a candidate query may take (solver.c; tests lower it through debug.c) */
+#define ASAM_CANDIDATE_BUDGET ((int64_t) 256 << 20)
+extern int64_t asam_candidate_budget;
+
 /* ---- solver context (solver.c) --------------------------------------------------------- */
 void asam_graph_forget(april_graph_t *g);
 /* graph.c: loss code and k of a factor; (0, 0) for factors without a robust loss */
 void asam_factor_loss(const april_graph_factor_t *f, int32_t *loss, double *k);
 /* graph.c: Jacobians of the xyt prediction (pose b in pose a's frame) at (pa, pb), row-major 3x3 */
 void asam_xyt_jacobians(const double *pa, const double *pb, double *Ja, double *Jb);
+/* graph.c: residual z - h(x) of an xyt factor at (pa, pb) and of an xytpos factor at pa, theta wrapped by mod2pi;
+ * the eval hooks and the candidate query share them */
+void asam_xyt_residual(const double *z, const double *pa, const double *pb, double *r);
+void asam_xytpos_residual(const double *z, const double *pa, double *r);
 /* serial.c */
 extern const stype_t stype_april_graph, stype_april_graph_attr, stype_april_node_xyt, stype_april_factor_xyt,
     stype_april_factor_xytpos, stype_april_factor_xyt_robust;

@@ -29,6 +29,30 @@ ASAM_API int asam_dbg_plan_marginal_paths(void *p, int n, const int *nodes, asam
     return rc;
 }
 
+/* plan_candidate_batches on a plan: returns the number of batches; batch_end / pose_end need k ints, poses 2k */
+ASAM_API int asam_dbg_plan_candidate_batches(void *p, int k, const int *a, const int *b, int64_t budget_doubles,
+                                             int *batch_end, int *poses, int *pose_end, int *ia, int *ib)
+{
+    int nb = 0;
+    plan_candidate_batches((const plan_t *) p, k, a, b, budget_doubles, batch_end, &nb, poses, pose_end, ia, ib);
+    return nb;
+}
+
+/* the residual helpers of graph.c: an xyt factor at (pa, pb), an xytpos factor at pa (pb NULL) */
+ASAM_API void asam_dbg_residual(const double *z, const double *pa, const double *pb, double *r)
+{
+    if (pb)
+        asam_xyt_residual(z, pa, pb, r);
+    else
+        asam_xytpos_residual(z, pa, r);
+}
+
+/* z scratch per batch of aprilsam_b200_candidate_mahalanobis in bytes; <= 0 restores the default */
+ASAM_API void asam_dbg_set_candidate_budget(int64_t bytes)
+{
+    asam_candidate_budget = bytes > 0 ? bytes : ASAM_CANDIDATE_BUDGET;
+}
+
 ASAM_API int asam_dbg_plan_build(void *p, int N, int F, const int *ftype, const int *fa, const int *fb)
 {
     return plan_build((plan_t *) p, NULL, N, F, ftype, fa, fb);

@@ -209,18 +209,29 @@ void asam_xyt_jacobians(const double *pa, const double *pb, double *Ja, double *
     memcpy(Jb, b, sizeof(b));
 }
 
+void asam_xyt_residual(const double *z, const double *pa, const double *pb, double *r)
+{
+    double ca = cos(pa[2]), sa = sin(pa[2]);
+    double dx = pb[0] - pa[0], dy = pb[1] - pa[1];
+    r[0] = z[0] - (ca * dx + sa * dy);
+    r[1] = z[1] - (-sa * dx + ca * dy);
+    r[2] = mod2pi(z[2] - (pb[2] - pa[2]));
+}
+
+void asam_xytpos_residual(const double *z, const double *pa, double *r)
+{
+    r[0] = z[0] - pa[0];
+    r[1] = z[1] - pa[1];
+    r[2] = mod2pi(z[2] - pa[2]);
+}
+
 static april_graph_factor_eval_t *xyt_eval_at(april_graph_factor_t *f, const double *pa, const double *pb,
                                               april_graph_factor_eval_t *ev)
 {
     if (!ev)
         ev = eval_alloc(2);
-    double ca = cos(pa[2]), sa = sin(pa[2]);
-    double dx = pb[0] - pa[0], dy = pb[1] - pa[1];
     asam_xyt_jacobians(pa, pb, ev->jacobians[0]->data, ev->jacobians[1]->data);
-    const double *z = f->u.common.z;
-    ev->r[0] = z[0] - (ca * dx + sa * dy);
-    ev->r[1] = z[1] - (-sa * dx + ca * dy);
-    ev->r[2] = mod2pi(z[2] - (pb[2] - pa[2]));
+    asam_xyt_residual(f->u.common.z, pa, pb, ev->r);
     eval_finish(ev, f->u.common.W);
     return ev;
 }
@@ -396,10 +407,7 @@ static april_graph_factor_eval_t *xytpos_eval(april_graph_factor_t *f, april_gra
         MATD_EL(ev->jacobians[0], i, i) = 1.0;
     april_graph_node_t *na;
     zarray_get(g->nodes, f->nodes[0], &na);
-    const double *z = f->u.common.z;
-    ev->r[0] = z[0] - na->state[0];
-    ev->r[1] = z[1] - na->state[1];
-    ev->r[2] = mod2pi(z[2] - na->state[2]);
+    asam_xytpos_residual(f->u.common.z, na->state, ev->r);
     eval_finish(ev, f->u.common.W);
     return ev;
 }

@@ -1944,3 +1944,62 @@ int plan_marginal_paths(const plan_t *pl, int n, const int *nodes, asam_marg_pat
     *hop_total = (int) hops;
     return 0;
 }
+
+/* doubles of query scratch (3 per scalar row of the root path) of the pose at elimination position q */
+static int64_t marginal_path_doubles(const plan_t *pl, int q)
+{
+    int64_t z = 0;
+    for (int s = pl->sn_of_q[q], js = 3 * (q - pl->desc[s].first); s >= 0; s = pl->desc[s].parent, js = 0)
+        z += 3 * (3 * (int64_t) pl->desc[s].cb - js);
+    return z;
+}
+
+/* scratch doubles of the poses of candidate (a, b) that the open batch does not hold yet (slot[node] < 0) */
+static int64_t candidate_new_doubles(const plan_t *pl, const int *slot, int a, int b)
+{
+    int64_t z = slot[a] < 0 ? marginal_path_doubles(pl, pl->node2q[a]) : 0;
+    if (b >= 0 && b != a && slot[b] < 0)
+        z += marginal_path_doubles(pl, pl->node2q[b]);
+    return z;
+}
+
+void plan_candidate_batches(const plan_t *pl, int k, const int *a, const int *b, int64_t budget, int *batch_end,
+                            int *n_batches, int *poses, int *pose_end, int *ia, int *ib)
+{
+    int *slot = malloc(sizeof(int) * (size_t) (pl->N > 0 ? pl->N : 1));
+    for (int i = 0; i < pl->N; i++)
+        slot[i] = -1;
+    int nb = 0, np = 0, p0 = 0, nc = 0; /* batches closed, poses listed, first pose of the open batch, its candidates */
+    int64_t z = 0;
+    for (int c = 0; c < k; c++) {
+        int64_t ext = candidate_new_doubles(pl, slot, a[c], b[c]);
+        if (nc > 0 && z + ext > budget) {
+            for (int i = p0; i < np; i++)
+                slot[poses[i]] = -1;
+            batch_end[nb] = c;
+            pose_end[nb++] = np;
+            p0 = np;
+            nc = 0;
+            z = 0;
+            ext = candidate_new_doubles(pl, slot, a[c], b[c]);
+        }
+        z += ext;
+        if (slot[a[c]] < 0) {
+            slot[a[c]] = np - p0;
+            poses[np++] = a[c];
+        }
+        ia[c] = slot[a[c]];
+        if (b[c] >= 0 && slot[b[c]] < 0) {
+            slot[b[c]] = np - p0;
+            poses[np++] = b[c];
+        }
+        ib[c] = b[c] >= 0 ? slot[b[c]] : -1;
+        nc++;
+    }
+    if (nc > 0) {
+        batch_end[nb] = k;
+        pose_end[nb++] = np;
+    }
+    free(slot);
+    *n_batches = nb;
+}

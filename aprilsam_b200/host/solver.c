@@ -1384,6 +1384,162 @@ ASAM_API int aprilsam_b200_marginal_covariance(april_graph_t *g, april_graph_cho
     return s ? marginal_run(s, n, nodes, out, fn) : -1;
 }
 
+/* ---- candidate factors: Sigma_rel and Mahalanobis distance (extension) ----------------------------------- */
+int64_t asam_candidate_budget = ASAM_CANDIDATE_BUDGET;
+
+/* J = [J_a J_b] (3 x 6, row-major) of an xyt factor between a and b at their l_points */
+static void candidate_jacobian(april_graph_t *g, int a, int b, double *J)
+{
+    double Ja[9], Jb[9];
+    asam_xyt_jacobians(node_at(g, a)->l_point, node_at(g, b)->l_point, Ja, Jb);
+    for (int r = 0; r < 3; r++)
+        for (int k = 0; k < 3; k++) {
+            J[6 * r + k] = Ja[3 * r + k];
+            J[6 * r + 3 + k] = Jb[3 * r + k];
+        }
+}
+
+/* Winv = W^-1 (exactly symmetric) by W = L L'; 0 unless W is exactly symmetric and positive definite */
+static int spd_inverse3(const double *W, double *Winv)
+{
+    for (int r = 0; r < 3; r++)
+        for (int c = r + 1; c < 3; c++)
+            if (!(W[3 * r + c] == W[3 * c + r]))
+                return 0;
+    double L[9] = { 0 }, X[9] = { 0 };
+    for (int j = 0; j < 3; j++) {
+        double d = W[4 * j];
+        for (int k = 0; k < j; k++)
+            d -= L[3 * j + k] * L[3 * j + k];
+        if (!(d > 0.0) || !isfinite(d))
+            return 0;
+        L[4 * j] = sqrt(d);
+        for (int i = j + 1; i < 3; i++) {
+            double v = W[3 * i + j];
+            for (int k = 0; k < j; k++)
+                v -= L[3 * i + k] * L[3 * j + k];
+            L[3 * i + j] = v / L[4 * j];
+        }
+    }
+    /* X = L^-1 (lower triangular), W^-1 = X' X */
+    for (int c = 0; c < 3; c++)
+        for (int i = c; i < 3; i++) {
+            double v = i == c ? 1.0 : 0.0;
+            for (int k = c; k < i; k++)
+                v -= L[3 * i + k] * X[3 * k + c];
+            X[3 * i + c] = v / L[4 * i];
+        }
+    for (int r = 0; r < 3; r++)
+        for (int c = r; c < 3; c++) {
+            double acc = 0.0;
+            for (int k = c; k < 3; k++)
+                acc += X[3 * k + r] * X[3 * k + c];
+            if (!isfinite(acc))
+                return 0;
+            Winv[3 * r + c] = Winv[3 * c + r] = acc;
+        }
+    return 1;
+}
+
+/* Sigma_rel (cov9, 9 doubles per candidate, may be NULL) and d2 of k candidates whose records hold J, r, Winv and
+ * has_w (ids checked by the caller).  Runs the batches of plan_candidate_batches, one asam_marginal_pairs each. */
+static int candidates_run(solver_t *s, int k, const int *a, const int *b, asam_marg_pair_t *rec, double *d2,
+                          double *cov9, const char *fn)
+{
+    const plan_t *pl = &s->plan;
+    int *batch_end = malloc(sizeof(int) * (size_t) k), *pose_end = malloc(sizeof(int) * (size_t) k);
+    int *poses = malloc(sizeof(int) * 2 * (size_t) k), *ia = malloc(sizeof(int) * (size_t) k);
+    int *ib = malloc(sizeof(int) * (size_t) k);
+    asam_marg_path_t *paths = malloc(sizeof(*paths) * 2 * (size_t) k);
+    double *out = malloc(sizeof(double) * 10 * (size_t) k);
+    int nb = 0, rc = 0;
+    plan_candidate_batches(pl, k, a, b, asam_candidate_budget / (int64_t) sizeof(double), batch_end, &nb, poses,
+                           pose_end, ia, ib);
+    for (int t = 0; t < nb && rc == 0; t++) {
+        const int c0 = t ? batch_end[t - 1] : 0, c1 = batch_end[t];
+        const int p0 = t ? pose_end[t - 1] : 0, n = pose_end[t] - p0;
+        int64_t z = 0;
+        int hops = 0;
+        if (plan_marginal_paths(pl, n, poses + p0, paths, &z, &hops) != 0) {
+            char why[512];
+            snprintf(why, sizeof(why), "%s", g_error);
+            asam_set_error("%s: %s", fn, why);
+            rc = -1;
+            break;
+        }
+        for (int c = c0; c < c1; c++) {
+            rec[c].pa = ia[c];
+            rec[c].pb = ib[c];
+        }
+        if (asam_marginal_pairs(s->gc->dev, n, paths, z, hops, pl->max_m, c1 - c0, rec + c0, out) != 0) {
+            asam_set_error("%s: %s", fn, asam_last_error());
+            rc = -1;
+            break;
+        }
+        for (int c = c0; c < c1; c++) {
+            d2[c] = out[10 * (size_t) (c - c0)];
+            if (cov9)
+                memcpy(cov9 + 9 * (size_t) c, out + 10 * (size_t) (c - c0) + 1, 9 * sizeof(double));
+        }
+    }
+    free(batch_end);
+    free(pose_end);
+    free(poses);
+    free(ia);
+    free(ib);
+    free(paths);
+    free(out);
+    return rc;
+}
+
+ASAM_API int aprilsam_b200_candidate_mahalanobis(april_graph_t *g, april_graph_cholesky_param_t *param, int k,
+                                                 const int *a, const int *b, const double *z, const double *W,
+                                                 double *d2, double *cov9)
+{
+    const char *fn = "aprilsam_b200_candidate_mahalanobis";
+    if (k < 1 || !a || !b || !z || !W || !d2) {
+        asam_set_error("%s: NULL a / b / z / W / d2 or k < 1", fn);
+        return -1;
+    }
+    solver_t *s = marginal_solver(g, param, fn);
+    if (!s)
+        return -1;
+    const int N = s->plan.N;
+    asam_marg_pair_t *rec = calloc((size_t) k, sizeof(*rec));
+    int rc = 0;
+    for (int c = 0; c < k && rc == 0; c++) {
+        const double *zc = z + 3 * (size_t) c;
+        rc = -1;
+        if (a[c] < 0 || a[c] >= N || b[c] >= N)
+            asam_set_error("%s: candidate %d: node %d is not in the solved graph (%d poses)", fn, c,
+                           a[c] < 0 || a[c] >= N ? a[c] : b[c], N);
+        else if (b[c] < -1)
+            asam_set_error("%s: candidate %d: b = %d; expected a pose id, or -1 for a prior on a", fn, c, b[c]);
+        else if (a[c] == b[c])
+            asam_set_error("%s: candidate %d: a == b (%d)", fn, c, a[c]);
+        else if (!isfinite(zc[0]) || !isfinite(zc[1]) || !isfinite(zc[2]))
+            asam_set_error("%s: candidate %d: z is not finite", fn, c);
+        else if (!spd_inverse3(W + 9 * (size_t) c, rec[c].Winv))
+            asam_set_error("%s: candidate %d: W is not symmetric positive definite", fn, c);
+        else
+            rc = 0;
+        if (rc)
+            break;
+        rec[c].has_w = 1;
+        const double *sa = node_at(g, a[c])->state;
+        if (b[c] >= 0) {
+            candidate_jacobian(g, a[c], b[c], rec[c].J);
+            asam_xyt_residual(zc, sa, node_at(g, b[c])->state, rec[c].r);
+        } else {
+            asam_xytpos_residual(zc, sa, rec[c].r);
+        }
+    }
+    if (rc == 0)
+        rc = candidates_run(s, k, a, b, rec, d2, cov9, fn);
+    free(rec);
+    return rc;
+}
+
 ASAM_API int aprilsam_b200_relative_covariance(april_graph_t *g, april_graph_cholesky_param_t *param, int a, int b,
                                                double out9[9])
 {
@@ -1395,35 +1551,17 @@ ASAM_API int aprilsam_b200_relative_covariance(april_graph_t *g, april_graph_cho
     solver_t *s = marginal_solver(g, param, fn);
     if (!s)
         return -1;
-    const int ids[2] = { a, b };
-    double S[36];
-    if (marginal_run(s, 2, ids, S, fn) != 0)
-        return -1;
-    /* J = [Ja Jb] of an xyt factor between a and b at the linearisation points; out = J S J' */
-    double J[18], Ja[9], Jb[9], JS[18];
-    asam_xyt_jacobians(node_at(g, a)->l_point, node_at(g, b)->l_point, Ja, Jb);
-    for (int r = 0; r < 3; r++)
-        for (int k = 0; k < 3; k++) {
-            J[6 * r + k] = Ja[3 * r + k];
-            J[6 * r + 3 + k] = Jb[3 * r + k];
+    for (int e = 0; e < 2; e++) {
+        const int id = e ? b : a;
+        if (id < 0 || id >= s->plan.N) {
+            asam_set_error("%s: node %d is not in the solved graph (%d poses)", fn, id, s->plan.N);
+            return -1;
         }
-    for (int r = 0; r < 3; r++)
-        for (int c = 0; c < 6; c++) {
-            double acc = 0.0;
-            for (int k = 0; k < 6; k++)
-                acc += J[6 * r + k] * S[6 * k + c];
-            JS[6 * r + c] = acc;
-        }
-    for (int r = 0; r < 3; r++)
-        for (int c = 0; c < 3; c++) {
-            double acc = 0.0;
-            for (int k = 0; k < 6; k++)
-                acc += JS[6 * r + k] * J[6 * c + k];
-            out9[3 * r + c] = acc;
-        }
-    /* exactly symmetric, like the covariance it comes from */
-    for (int r = 0; r < 3; r++)
-        for (int c = r + 1; c < 3; c++)
-            out9[3 * c + r] = out9[3 * r + c];
-    return 0;
+    }
+    /* one candidate without W: Sigma_rel only */
+    asam_marg_pair_t rec;
+    memset(&rec, 0, sizeof(rec));
+    candidate_jacobian(g, a, b, rec.J);
+    double d2;
+    return candidates_run(s, 1, &a, &b, &rec, &d2, out9, fn);
 }

@@ -527,7 +527,8 @@ H_EXPORT void h_set_policy_ratio(hctx_t *h, double ratio)
 #endif
 }
 
-/* aprilsam_b200_marginal_covariance / _relative_covariance (extensions; absent from the reference build) */
+/* aprilsam_b200_marginal_covariance / _relative_covariance / _candidate_mahalanobis (extensions; absent from the
+ * reference build) */
 #ifndef HARNESS_REFERENCE
 H_EXPORT int h_marginal_cov(hctx_t *h, int n, const int *nodes, double *out)
 {
@@ -537,6 +538,12 @@ H_EXPORT int h_marginal_cov(hctx_t *h, int n, const int *nodes, double *out)
 H_EXPORT int h_relative_cov(hctx_t *h, int a, int b, double *out9)
 {
     return aprilsam_b200_relative_covariance(h->g, h->p, a, b, out9);
+}
+
+H_EXPORT int h_candidate_mahalanobis(hctx_t *h, int k, const int *a, const int *b, const double *z, const double *W,
+                                     double *d2, double *cov9)
+{
+    return aprilsam_b200_candidate_mahalanobis(h->g, h->p, k, a, b, z, W, d2, cov9);
 }
 #endif
 

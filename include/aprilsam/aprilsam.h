@@ -287,6 +287,28 @@ int aprilsam_b200_marginal_covariance(april_graph_t *graph, april_graph_cholesky
  * marginal of (a, b) and J = [J_a J_b] the Jacobians of an xyt factor between a and b at their l_points. */
 int aprilsam_b200_relative_covariance(april_graph_t *graph, april_graph_cholesky_param_t *param, int a, int b,
                                       double out9[9]);
+/* Mahalanobis distances of k candidate factors against the last solve, for gating loop closures.  Candidate c is
+ * the factor the caller would add: an xyt factor between poses a[c] and b[c] (b[c] >= 0), or a prior (xytpos) on
+ * pose a[c] (b[c] == -1), with measurement z (3k doubles) and information matrix W (9k doubles, row-major), the
+ * same z and W that april_graph_factor_xyt_create / _xytpos_create take.  With r the factor's residual at the
+ * current states (theta wrapped by mod2pi, as the eval hooks compute it) and
+ *   Sigma_rel = J Sigma_ab J'  (J = [J_a J_b] at the l_points: exactly aprilsam_b200_relative_covariance(a, b))
+ *   Sigma_rel = Sigma_aa       (a prior: the diagonal block of aprilsam_b200_marginal_covariance)
+ * d2[c] = r' (Sigma_rel + W^-1)^-1 r, NaN if Sigma_rel + W^-1 is not numerically positive definite.  A caller
+ * accepts a candidate when d2 is below a chi-square quantile with 3 degrees of freedom, for example 7.815 (95 %)
+ * or 11.345 (99 %).  Without a prior in the graph Sigma_aa is mostly 1/tikhanov, so prior candidates are only
+ * meaningful on graphs that hold a prior.
+ *
+ * cov9 (NULL allowed): Sigma_rel of every candidate, 9 doubles row-major, exactly symmetric.  A candidate's d2 and
+ * Sigma_rel are the same alone or in any request, in any order, and from call to call.  The cost follows the
+ * distinct poses: a pose that appears in many candidates is walked once.
+ *
+ * Returns 0, or -1 with the reason in aprilsam_b200_last_error() for the cases of the covariance queries above, and
+ * for k < 1, NULL a / b / z / W / d2, b[c] < -1, a[c] == b[c], a non-finite z or a W that is not exactly symmetric
+ * and positive definite; the message names the index of the candidate at fault.  d2 and cov9 are unspecified after
+ * an error; the solver stays usable. */
+int aprilsam_b200_candidate_mahalanobis(april_graph_t *graph, april_graph_cholesky_param_t *param, int k, const int *a,
+                                        const int *b, const double *z, const double *W, double *d2, double *cov9);
 
 /* Relinearisation / re-ordering policy of april_graph_cholesky_inc().  The reference escalates an
  * incremental step to a full batch solve when `start_over > nthreshold` (kept) and, as shipped, also

@@ -189,6 +189,24 @@ typedef struct asam_marg_path {
  * first call.  One synchronisation. */
 int asam_marginal_cov(asam_dev_t *d, int n, const asam_marg_path_t *paths, int64_t z_doubles, int n_hops, int max_m,
                       double *out);
+/* One candidate factor of asam_marginal_pairs: an xyt factor between the poses of paths[pa] and paths[pb], or a
+ * prior on paths[pa] (pb = -1).  J = [J_a J_b] (3 x 6, row-major) at the l_points, r the residual at the states,
+ * Winv the inverse of the factor's information matrix (exactly symmetric); has_w = 0: no W, d2 is NaN. */
+typedef struct asam_marg_pair {
+    int32_t pa, pb;
+    int32_t has_w, pad;
+    double J[18];
+    double r[3];
+    double Winv[9];
+} asam_marg_pair_t;
+/* k_marginal_path over the n distinct poses, then one CTA per candidate (k_marginal_pairs): the 3 x 3 blocks
+ * Sigma_aa, Sigma_ab, Sigma_bb (bit-identical to the blocks of asam_marginal_cov), Sigma_rel = J Sigma_6 J' (Sigma_aa
+ * for a prior), S = Sigma_rel + Winv and d2 = r' S^-1 r by a 3 x 3 Cholesky of S (NaN for a non-positive pivot).
+ * out: 10 doubles per candidate, {d2, Sigma_rel (row-major, exactly symmetric)}, host memory.  A candidate's
+ * output depends only on its own record.  Writes only the scratch buffer; one H2D copy per table and one
+ * synchronisation. */
+int asam_marginal_pairs(asam_dev_t *d, int n, const asam_marg_path_t *paths, int64_t z_doubles, int n_hops, int max_m,
+                        int k, const asam_marg_pair_t *pairs, double *out);
 
 /* chi2 = sum 0.5 r'Wr (xyt, at state) + sum 0.5 rho(r'Wr) (robust xyt) + sum r'Wr (xytpos) over factors [0, n_factors)
  * using the st mirror (april_graph.c:79-98). Deterministic reduction. */
@@ -218,6 +236,8 @@ int asam_debug_read_buffer(asam_dev_t *d, int id, int64_t off, int64_t bytes, vo
 /* Byte offsets in the scratch of an asam_marginal_cov call with these arguments: {out (3n x 3n doubles), paths,
  * z, hops (4 ints each: supernode, js, c, offset of its rows from the pose's zoff), total}; the error word is at 0. */
 void asam_debug_marginal_layout(int n, int64_t z_doubles, int n_hops, int64_t out5[5]);
+/* The same for an asam_marginal_pairs call: {out (10 doubles per candidate), paths, z, hops, pairs, total}. */
+void asam_debug_marginal_pairs_layout(int n, int64_t z_doubles, int n_hops, int k, int64_t out6[6]);
 int asam_sync(asam_dev_t *d);
 /* Counters: [0] kernel launches since creation, [1] bytes H2D, [2] bytes D2H. */
 int asam_counters(asam_dev_t *d, int64_t *out3);
