@@ -280,13 +280,6 @@ static int leaf_max_m_for(int nsn)
     return nsn >= ASAM_LEAF_WIDE_MIN_SN ? ASAM_LEAF_MAX_M_DEFAULT : 48;
 }
 
-static double host_now_ms(void)
-{
-    struct timespec ts;
-    clock_gettime(CLOCK_MONOTONIC, &ts);
-    return ts.tv_sec * 1e3 + ts.tv_nsec * 1e-6;
-}
-
 static double host_spin(int iters)
 {
     volatile double x = 1.0;
@@ -305,15 +298,15 @@ int asam_host_threads(void)
         if (want > 1) {
             /* two threads spinning for a fixed count each: side by side that takes as long as one of them */
             const int iters = 40000;
-            double t0 = host_now_ms();
+            double t0 = pp_now();
             host_spin(iters);
-            const double t1 = host_now_ms() - t0;
+            const double t1 = pp_now() - t0;
             double tp = 1e30;
             for (int rep = 0; rep < 3 && tp > 2.5 * t1 + 0.05; rep++) { /* (the first region also creates the threads) */
-                t0 = host_now_ms();
+                t0 = pp_now();
 #pragma omp parallel num_threads(2)
                 host_spin(iters);
-                const double t = host_now_ms() - t0;
+                const double t = pp_now() - t0;
                 tp = t < tp ? t : tp;
             }
             if (tp > 2.5 * t1 + 0.05)
@@ -325,8 +318,6 @@ int asam_host_threads(void)
     }
     return v;
 }
-
-static int plan_threads(void) { return asam_host_threads(); }
 
 static int compute_rel(plan_t *pl, int s)
 {
@@ -1029,92 +1020,161 @@ static void build_schedule(plan_t *pl)
     free(owner);
 }
 
-/* ---- batch build --------------------------------------------------------------------------- */
-static int plan_build_impl(plan_t *pl, asam_dev_t *dev, int N, int n_factors, const int *ftype, const int *fa,
-                           const int *fb, const int *order_keep, int N_keep)
+/* ---- decisions shared by the batch build and the incremental append ------------------------------ */
+/* Factors [f0, n_factors) on poses [0, N): a prior on one pose, or a two-pose factor on two distinct poses.  Returns 0,
+ * 1 (error text set), or 2 for a two-pose factor between two poses below N0, which no incremental step can append. */
+static int check_factors(int f0, int n_factors, int N, int N0, const int *ftype, const int *fa, const int *fb)
 {
-    uint64_t keep_hash = pl->struct_hash;
-    int keep_world = pl->world, keep_rank = pl->rank, keep_team = pl->max_team, keep_cta = pl->n_cta;
-    plan_free(pl);
-    pl->struct_hash = keep_hash;
-    pl->world = keep_world;
-    pl->rank = keep_rank;
-    pl->max_team = keep_team;
-    pl->n_cta = keep_cta;
-    if (dev) { /* teams are sized for the CTAs this device actually seats (MIG slice, smaller part, ...) */
-        int n_sm = 0, fac_grid = 0, fac_smem = 0, bs_grid = 0;
-        if (asam_device_info(dev, &n_sm, &fac_grid, &fac_smem, &bs_grid) == 0 && fac_grid > 0)
-            pl->max_team = fac_grid < 120 ? fac_grid : 120, pl->n_cta = fac_grid;
-    }
-    if (N <= 0)
-        return 0;
-    node_arrays_reserve(pl, N);
-    fslot_reserve(pl, n_factors);
-    pl->N = N;
-    pl->n_factors = n_factors;
-
-    double bt_ = pp_now(), bt2_;
-#define BUILD_LAP(i)                 \
-    do {                             \
-        bt2_ = pp_now();             \
-        g_build_prof[i] += bt2_ - bt_; \
-        bt_ = bt2_;                  \
-    } while (0)
-    /* 1. unique node pairs -> Hessian slots */
-    pairmap_init(&pl->pairs, n_factors);
-    ivec_t plo = { 0 }, phi = { 0 };
-    for (int f = 0; f < n_factors; f++) {
+    for (int f = f0; f < n_factors; f++) {
         if (asam_two_pose_type(ftype[f])) {
-            int a = fa[f], b = fb[f];
-            if (a == b || a < 0 || b < 0 || a >= N || b >= N) {
-                asam_set_error("factor %d: bad node ids (%d,%d)", f, a, b);
+            if (fa[f] == fb[f] || fa[f] < 0 || fb[f] < 0 || fa[f] >= N || fb[f] >= N) {
+                asam_set_error("factor %d: bad node ids (%d,%d)", f, fa[f], fb[f]);
                 return 1;
             }
-            int lo = a < b ? a : b, hi = a < b ? b : a, created;
-            int slot = pairmap_get_or_add(&pl->pairs, lo, hi, pl->n_slots, &created);
-            if (created) {
-                ivec_push(&plo, lo);
-                ivec_push(&phi, hi);
-                pl->n_slots++;
-            }
-            pl->fslot[f] = slot;
+            if (fa[f] < N0 && fb[f] < N0)
+                return 2;
         } else if (ftype[f] == APRIL_GRAPH_FACTOR_XYTPOS_TYPE) {
             if (fa[f] < 0 || fa[f] >= N) {
                 asam_set_error("factor %d: bad node id %d", f, fa[f]);
                 return 1;
             }
-            pl->fslot[f] = -1;
         } else {
             asam_set_error("factor %d: unsupported factor type %d", f, ftype[f]);
             return 1;
         }
     }
-    const int S = pl->n_slots;
+    return 0;
+}
 
-    /* 2. adjacency CSR, ascending */
-    int *adj_ptr = calloc((size_t) N + 1, sizeof(int));
+/* Hessian slots of the checked factors [f0, n_factors): one per distinct pose pair, -1 for a prior.  The pairs that
+ * get a new slot are appended to (plo, phi) in slot order. */
+static void assign_slots(plan_t *pl, int f0, int n_factors, const int *ftype, const int *fa, const int *fb, ivec_t *plo,
+                         ivec_t *phi)
+{
+    fslot_reserve(pl, n_factors);
+    for (int f = f0; f < n_factors; f++) {
+        if (!asam_two_pose_type(ftype[f])) {
+            pl->fslot[f] = -1;
+            continue;
+        }
+        int a = fa[f], b = fb[f], lo = a < b ? a : b, hi = a < b ? b : a, created;
+        int slot = pairmap_get_or_add(&pl->pairs, lo, hi, pl->n_slots, &created);
+        if (created) {
+            ivec_push(plo, lo);
+            ivec_push(phi, hi);
+            pl->n_slots++;
+        }
+        pl->fslot[f] = slot;
+    }
+}
+
+/* A new supernode whose one column is position q, without a parent; returns its id. */
+static int sn_create(plan_t *pl, int q)
+{
+    sn_arrays_reserve(pl, pl->nsn + 1);
+    pl->desc[pl->nsn] = (asam_sn_desc_t) { .first = q, .cb = 1, .parent = -1 };
+    return pl->nsn++;
+}
+
+/* Block rows of supernode s from its row list; the largest front order follows. */
+static void sn_set_mb(plan_t *pl, int s)
+{
+    pl->desc[s].mb = pl->snh[s].rows.n;
+    if (3 * pl->desc[s].mb > pl->max_m)
+        pl->max_m = 3 * pl->desc[s].mb;
+}
+
+/* Places the front of supernode s at the end of the arena, with room for a front of mb_capacity block rows. */
+static void front_place(plan_t *pl, int s, int mb_capacity)
+{
+    pl->desc[s].f_off = pl->arena_n;
+    pl->desc[s].reserved = front_doubles(mb_capacity);
+    pl->arena_n += pl->desc[s].reserved;
+}
+
+/* Supernode s is in the back-solve leaf set but no longer fits k_backsolve_leaf. */
+static int bs_leaf_outgrown(const plan_t *pl, int s)
+{
+    const asam_sn_desc_t *d = &pl->desc[s];
+    return pl->n_bs_leaf > 0 && pl->bs_leaf[s] &&
+           (3 * d->cb > ASAM_BSLEAF_MAX || 3 * (d->mb - d->cb) > ASAM_BSLEAF_MAX);
+}
+
+/* Where the Hessian block of poses (lo, hi) goes: the supernode of the pose eliminated first (returned), its column *cb
+ * there, and *rb, the block row of the other pose (-1: none), with ASAM_TR_FLAG where the slot is read transposed. */
+static int gather_find(const plan_t *pl, int lo, int hi, int *rb, int *cb)
+{
+    int qlo = pl->node2q[lo], qhi = pl->node2q[hi];
+    int qe = qlo < qhi ? qlo : qhi, ql = qlo < qhi ? qhi : qlo;
+    int s = pl->sn_of_q[qe];
+    const sn_host_t *h = &pl->snh[s];
+    *rb = find_sorted(h->rows.p, h->rows.n, ql) | (qe == qlo ? 0 : ASAM_TR_FLAG);
+    *cb = qe - pl->desc[s].first;
+    return s;
+}
+
+static void gather_push(plan_t *pl, int s, int slot, int rb, int cb)
+{
+    sn_host_t *h = &pl->snh[s];
+    ivec_push(&h->a_slot, slot);
+    ivec_push(&h->a_rb, rb);
+    ivec_push(&h->a_cb, cb);
+}
+
+/* ---- batch build --------------------------------------------------------------------------- */
+static void build_lap(int i, double *t)
+{
+    const double now = pp_now();
+    g_build_prof[i] += now - *t;
+    *t = now;
+}
+
+/* Empties the plan for a rebuild.  What survives it: the structure hash and where the plan runs (world, rank, the
+ * largest team and the resident CTAs, re-read from `dev` when there is one). */
+static void plan_reset(plan_t *pl, asam_dev_t *dev)
+{
+    const uint64_t hash = pl->struct_hash;
+    const int world = pl->world, rank = pl->rank, max_team = pl->max_team, n_cta = pl->n_cta;
+    plan_free(pl);
+    pl->struct_hash = hash;
+    pl->world = world, pl->rank = rank;
+    pl->max_team = max_team, pl->n_cta = n_cta;
+    if (dev) { /* teams are sized for the CTAs this device actually seats (MIG slice, smaller part, ...) */
+        int n_sm = 0, fac_grid = 0, fac_smem = 0, bs_grid = 0;
+        if (asam_device_info(dev, &n_sm, &fac_grid, &fac_smem, &bs_grid) == 0 && fac_grid > 0)
+            pl->max_team = fac_grid < 120 ? fac_grid : 120, pl->n_cta = fac_grid;
+    }
+}
+
+/* Adjacency of the N poses from the slots' pose pairs, CSR with ascending lists (malloc'd) */
+static void adjacency(int N, const ivec_t *plo, const ivec_t *phi, int **adj_ptr_out, int **adj_out)
+{
+    const int S = plo->n;
+    int *adj_ptr = *adj_ptr_out = calloc((size_t) N + 1, sizeof(int));
     for (int s = 0; s < S; s++) {
-        adj_ptr[plo.p[s] + 1]++;
-        adj_ptr[phi.p[s] + 1]++;
+        adj_ptr[plo->p[s] + 1]++;
+        adj_ptr[phi->p[s] + 1]++;
     }
     for (int i = 0; i < N; i++)
         adj_ptr[i + 1] += adj_ptr[i];
-    int *adj = malloc(sizeof(int) * (size_t) (2 * S + 1));
-    int *fill = malloc(sizeof(int) * (size_t) N);
+    int *adj = *adj_out = malloc(sizeof(int) * (size_t) (2 * S + 1)), *fill = malloc(sizeof(int) * (size_t) N);
     memcpy(fill, adj_ptr, sizeof(int) * (size_t) N);
     for (int s = 0; s < S; s++) {
-        adj[fill[plo.p[s]]++] = phi.p[s];
-        adj[fill[phi.p[s]]++] = plo.p[s];
+        adj[fill[plo->p[s]]++] = phi->p[s];
+        adj[fill[phi->p[s]]++] = plo->p[s];
     }
     for (int i = 0; i < N; i++)
         sort_ints(adj + adj_ptr[i], adj_ptr[i + 1] - adj_ptr[i]);
     free(fill);
+}
 
-    BUILD_LAP(0); /* slots + adjacency */
-    /* 3. elimination order */
+/* pl->order and pl->pos: the reference's elimination order, or order_keep for the first N_keep positions and the
+ * other poses after them in id order */
+static void elimination_order(plan_t *pl, const int *adj_ptr, const int *adj, const int *order_keep, int N_keep)
+{
+    const int N = pl->N;
     if (order_keep) {
-        for (int p = 0; p < N_keep; p++)
-            pl->order[p] = order_keep[p];
+        memcpy(pl->order, order_keep, sizeof(int) * (size_t) N_keep);
         for (int p = N_keep; p < N; p++)
             pl->order[p] = p;
     } else {
@@ -1124,13 +1184,24 @@ static int plan_build_impl(plan_t *pl, asam_dev_t *dev, int N, int n_factors, co
     }
     for (int p = 0; p < N; p++)
         pl->pos[pl->order[p]] = p;
+}
 
-    BUILD_LAP(1); /* ordering */
-    /* 4. block symbolic factorisation in reference positions */
-    int *parent = pl->parent_pos;
+/* Block elimination tree in reference positions p; the parents are pl->parent_pos.  The rows below column p are
+ * bl[bptr[p] .. bptr[p+1]), unsorted: only their sizes, their union and their minimum (the parent) are used, and the
+ * rows of a supernode are sorted once, in numeric positions, by sn_structure().  The children of p are head[p],
+ * next[head[p]], ... (-1 ends the list).  post_order() numbers the tree: qpos[p] = q, pofq[q] = p. */
+typedef struct {
+    int64_t *bptr;
+    ivec_t bl;
+    int *head, *next;
+    int *qpos, *pofq;
+} etree_t;
+
+static etree_t block_symbolic(plan_t *pl, const int *adj_ptr, const int *adj)
+{
+    const int N = pl->N;
     int *head = malloc(sizeof(int) * (size_t) N), *tail = malloc(sizeof(int) * (size_t) N);
-    int *next = malloc(sizeof(int) * (size_t) N), *nchild = calloc((size_t) N, sizeof(int));
-    int *stamp = calloc((size_t) N, sizeof(int));
+    int *next = malloc(sizeof(int) * (size_t) N), *stamp = calloc((size_t) N, sizeof(int));
     int64_t *bptr = malloc(sizeof(int64_t) * ((size_t) N + 1));
     ivec_t bl = { 0 };
     for (int p = 0; p < N; p++)
@@ -1155,110 +1226,96 @@ static int plan_build_impl(plan_t *pl, asam_dev_t *dev, int N, int n_factors, co
                 }
             }
         }
-        /* (the lists stay unsorted: only their sizes, their union and their minimum -- the parent -- are used; the
-         * rows of a supernode are sorted once, in numeric positions, in step 7) */
         bptr[p + 1] = bl.n;
         int pmin = -1;
         for (int e = start; e < bl.n; e++)
             if (pmin < 0 || bl.p[e] < pmin)
                 pmin = bl.p[e];
-        parent[p] = pmin;
-        if (parent[p] >= 0) {
-            int P = parent[p];
-            if (tail[P] < 0)
-                head[P] = p;
+        pl->parent_pos[p] = pmin;
+        if (pmin >= 0) { /* p is the last child of pmin so far */
+            if (tail[pmin] < 0)
+                head[pmin] = p;
             else
-                next[tail[P]] = p;
-            tail[P] = p;
-            nchild[P]++;
+                next[tail[pmin]] = p;
+            tail[pmin] = p;
         }
     }
-    free(stamp);
-    free(adj);
-    free(adj_ptr);
+    free(tail); free(stamp);
+    return (etree_t) { .bptr = bptr, .bl = bl, .head = head, .next = next };
+}
 
-    BUILD_LAP(2); /* block symbolic */
-    /* 5. post-order -> numeric positions q.  Children are visited in ascending structure
-     * size so that the child with the largest front is numbered right before its parent and can
-     * share a supernode with it (step 6). */
-    {
-        int *kids = malloc(sizeof(int) * (size_t) N);
-        for (int p = 0; p < N; p++) {
-            int n = 0;
-            for (int c = head[p]; c >= 0; c = next[c])
-                kids[n++] = c;
-            if (n < 2)
-                continue;
-            for (int i = 1; i < n; i++) { /* insertion sort by (|below|, position) */
-                int v = kids[i], j = i - 1;
-                int64_t kv = bptr[v + 1] - bptr[v];
-                while (j >= 0 && (bptr[kids[j] + 1] - bptr[kids[j]]) > kv) {
-                    kids[j + 1] = kids[j];
-                    j--;
-                }
-                kids[j + 1] = v;
+/* Post-order of the tree -> numeric positions q (t->qpos, t->pofq, pl->node2q, pl->q2node).  Children are visited in
+ * ascending structure size so that the child with the largest front is numbered right before its parent and can
+ * share a supernode with it (supernodes()).  Uses up the child lists. */
+static void post_order(plan_t *pl, etree_t *t)
+{
+    const int N = pl->N;
+    int *head = t->head, *next = t->next;
+    const int64_t *bptr = t->bptr;
+    int *kids = malloc(sizeof(int) * (size_t) N);
+    for (int p = 0; p < N; p++) {
+        int n = 0;
+        for (int c = head[p]; c >= 0; c = next[c])
+            kids[n++] = c;
+        if (n < 2)
+            continue;
+        for (int i = 1; i < n; i++) { /* insertion sort by (|below|, position) */
+            int v = kids[i], j = i - 1;
+            int64_t kv = bptr[v + 1] - bptr[v];
+            while (j >= 0 && (bptr[kids[j] + 1] - bptr[kids[j]]) > kv) {
+                kids[j + 1] = kids[j];
+                j--;
             }
-            head[p] = kids[0];
-            for (int i = 0; i + 1 < n; i++)
-                next[kids[i]] = kids[i + 1];
-            next[kids[n - 1]] = -1;
-            tail[p] = kids[n - 1];
+            kids[j + 1] = v;
         }
-        free(kids);
+        head[p] = kids[0];
+        for (int i = 0; i + 1 < n; i++)
+            next[kids[i]] = kids[i + 1];
+        next[kids[n - 1]] = -1;
     }
-    int *qpos = malloc(sizeof(int) * (size_t) N), *pofq = malloc(sizeof(int) * (size_t) N);
-    {
-        int *stack = malloc(sizeof(int) * (size_t) N), *it = malloc(sizeof(int) * (size_t) N);
-        int q = 0;
-        for (int r = 0; r < N; r++) {
-            if (parent[r] >= 0)
-                continue;
-            int sp = 0;
-            stack[sp] = r;
-            it[sp] = head[r];
-            sp++;
-            while (sp > 0) {
-                int c = it[sp - 1];
-                if (c >= 0) {
-                    it[sp - 1] = next[c];
-                    stack[sp] = c;
-                    it[sp] = head[c];
-                    sp++;
-                } else {
-                    int p = stack[--sp];
-                    qpos[p] = q;
-                    pofq[q] = p;
-                    q++;
-                }
+    free(kids);
+    int *qpos = t->qpos = malloc(sizeof(int) * (size_t) N), *pofq = t->pofq = malloc(sizeof(int) * (size_t) N);
+    int *stack = malloc(sizeof(int) * (size_t) N), q = 0;
+    for (int r = 0; r < N; r++) {
+        if (pl->parent_pos[r] >= 0)
+            continue;
+        int sp = 0;
+        stack[0] = r;
+        while (sp >= 0) { /* head[p]: the next child of p to visit */
+            int p = stack[sp], c = head[p];
+            if (c >= 0) {
+                head[p] = next[c];
+                stack[++sp] = c;
+            } else {
+                sp--;
+                qpos[p] = q;
+                pofq[q++] = p;
             }
         }
-        free(stack);
-        free(it);
     }
+    free(stack);
     for (int p = 0; p < N; p++) {
         pl->node2q[pl->order[p]] = qpos[p];
         pl->q2node[qpos[p]] = pl->order[p];
     }
+}
 
-    /* 6. supernodes: a node joins the supernode of the child numbered right before it when the
-     * child's structure is the node's structure plus itself (fundamental), or misses at most
-     * RELAX_Z block rows of it (relaxed amalgamation: a few explicit zero blocks buy fewer, fatter
-     * fronts and a shorter dependency chain); width capped at MAX_SN_COLS. */
-    int relax_z = RELAX_Z, relax_fill = RELAX_FILL; /* ASAM_RELAX_Z / ASAM_RELAX_FILL override (tuning) */
-    if (getenv("ASAM_RELAX_Z"))
-        relax_z = atoi(getenv("ASAM_RELAX_Z"));
-    if (getenv("ASAM_RELAX_FILL"))
-        relax_fill = atoi(getenv("ASAM_RELAX_FILL"));
-    int team_merge_pct = TEAM_MERGE_PCT;
-    double team_merge_mflop = TEAM_MERGE_MFLOP;
-    if (getenv("ASAM_TEAM_MERGE_PCT"))
-        team_merge_pct = atoi(getenv("ASAM_TEAM_MERGE_PCT"));
-    if (getenv("ASAM_TEAM_MERGE_MFLOP"))
-        team_merge_mflop = atof(getenv("ASAM_TEAM_MERGE_MFLOP"));
-    pl->nsn = 0;
-    pl->nnz_l_blocks = 0;
-    pl->flops = 0.0;
-    for (int q = 0; q < N; q++) {
+/* Supernodes (and the statistics nnz_l_blocks, flops): a node joins the supernode of the child numbered right before
+ * it when the child's structure is the node's structure plus itself (fundamental), or misses at most RELAX_Z block
+ * rows of it (relaxed amalgamation: a few explicit zero blocks buy fewer, fatter fronts and a shorter dependency
+ * chain); width capped at MAX_SN_COLS. */
+static void supernodes(plan_t *pl, const etree_t *t)
+{
+    const int64_t *bptr = t->bptr;
+    const int *pofq = t->pofq;
+    const int *parent = pl->parent_pos;
+    /* ASAM_RELAX_Z, ASAM_RELAX_FILL, ASAM_TEAM_MERGE_PCT and ASAM_TEAM_MERGE_MFLOP override (tuning) */
+    const int relax_z = getenv("ASAM_RELAX_Z") ? atoi(getenv("ASAM_RELAX_Z")) : RELAX_Z;
+    const int relax_fill = getenv("ASAM_RELAX_FILL") ? atoi(getenv("ASAM_RELAX_FILL")) : RELAX_FILL;
+    const int team_merge_pct = getenv("ASAM_TEAM_MERGE_PCT") ? atoi(getenv("ASAM_TEAM_MERGE_PCT")) : TEAM_MERGE_PCT;
+    const double team_merge_mflop =
+        getenv("ASAM_TEAM_MERGE_MFLOP") ? atof(getenv("ASAM_TEAM_MERGE_MFLOP")) : TEAM_MERGE_MFLOP;
+    for (int q = 0; q < pl->N; q++) {
         int p = pofq[q];
         int nb = (int) (bptr[p + 1] - bptr[p]);
         pl->nnz_l_blocks += 1 + nb;
@@ -1289,26 +1346,21 @@ static int plan_build_impl(plan_t *pl, asam_dev_t *dev, int N, int n_factors, co
                 27.0 * gcb * z * (2.0 * (gcb + nbp) + z) <= 1e6 * team_merge_mflop)
                 merge = 1;
         }
-        if (merge) {
+        if (merge)
             pl->desc[pl->nsn - 1].cb++;
-        } else {
-            sn_arrays_reserve(pl, pl->nsn + 1);
-            asam_sn_desc_t *d = &pl->desc[pl->nsn];
-            memset(d, 0, sizeof(*d));
-            d->first = q;
-            d->cb = 1;
-            d->parent = -1;
-            pl->nsn++;
-        }
+        else
+            sn_create(pl, q);
         pl->sn_of_q[q] = pl->nsn - 1;
     }
+}
 
-    BUILD_LAP(3); /* post-order + supernodes */
-    /* 7. row lists, parents, children, levels */
-    pl->max_m = 0;
-    int max_m = 0;
+/* Row lists, block rows, parents, children, levels and relative indices of every supernode */
+static int sn_structure(plan_t *pl, const etree_t *t)
+{
+    const int64_t *bptr = t->bptr;
+    const int *qpos = t->qpos, *pofq = t->pofq;
     /* (per-supernode work, independent: split over a few host threads on large graphs, like the pose loops of solver.c) */
-#pragma omp parallel for schedule(static, 256) reduction(max : max_m) if (pl->nsn >= PLAN_OMP_MIN_SN) num_threads(plan_threads())
+#pragma omp parallel for schedule(static, 256) if (pl->nsn >= PLAN_OMP_MIN_SN) num_threads(asam_host_threads())
     for (int s = 0; s < pl->nsn; s++) {
         asam_sn_desc_t *d = &pl->desc[s];
         sn_host_t *h = &pl->snh[s];
@@ -1318,16 +1370,13 @@ static int plan_build_impl(plan_t *pl, asam_dev_t *dev, int N, int n_factors, co
         for (int k = 0; k < d->cb; k++)
             ivec_push(&h->rows, d->first + k);
         for (int64_t e = bptr[pt]; e < bptr[pt + 1]; e++)
-            ivec_push(&h->rows, qpos[bl.p[e]]);
+            ivec_push(&h->rows, qpos[t->bl.p[e]]);
         /* positions on a root path are ordered alike in both numberings; be safe anyway */
         sort_ints(h->rows.p + d->cb, nb);
-        d->mb = h->rows.n;
-        if (3 * d->mb > max_m)
-            max_m = 3 * d->mb;
         d->parent = nb > 0 ? pl->sn_of_q[h->rows.p[d->cb]] : -1;
     }
-    pl->max_m = max_m;
     for (int s = 0; s < pl->nsn; s++) {
+        sn_set_mb(pl, s);
         int P = pl->desc[s].parent;
         if (P >= 0) {
             ivec_push(&pl->snh[P].children, s);
@@ -1336,95 +1385,54 @@ static int plan_build_impl(plan_t *pl, asam_dev_t *dev, int N, int n_factors, co
                 pl->desc[P].level = lv; /* children have smaller ids: final when P is reached */
         }
     }
-    pl->n_levels = 0;
-    {
-        int rel_bad = 0, n_levels = 0;
-#pragma omp parallel for schedule(static, 256) reduction(| : rel_bad) reduction(max : n_levels) if (pl->nsn >= PLAN_OMP_MIN_SN) num_threads(plan_threads())
-        for (int s = 0; s < pl->nsn; s++) {
-            rel_bad |= compute_rel(pl, s);
-            if (pl->desc[s].level + 1 > n_levels)
-                n_levels = pl->desc[s].level + 1;
-        }
-        if (rel_bad)
-            return 1;
-        pl->n_levels = n_levels;
-    }
-    free(bptr);
-    ivec_free(&bl);
-    free(head);
-    free(tail);
-    free(next);
-    free(nchild);
-    free(qpos);
-    free(pofq);
-
-    BUILD_LAP(4); /* row lists, rel */
-    /* 8. Hessian gather lists: the searches in parallel, the lists filled in slot order */
-    {
-        int *g_sn = malloc(sizeof(int) * (size_t) (S + 1)), *g_rb = malloc(sizeof(int) * (size_t) (S + 1)),
-            *g_cb = malloc(sizeof(int) * (size_t) (S + 1));
-        int bad_slot = -1;
-#pragma omp parallel for schedule(static, 4096) reduction(max : bad_slot) if (S >= 8 * PLAN_OMP_MIN_SN) num_threads(plan_threads())
-        for (int sl = 0; sl < S; sl++) {
-            int lo = plo.p[sl], hi = phi.p[sl];
-            int qlo = pl->node2q[lo], qhi = pl->node2q[hi];
-            int qe = qlo < qhi ? qlo : qhi, ql = qlo < qhi ? qhi : qlo;
-            int s = pl->sn_of_q[qe];
-            const sn_host_t *h = &pl->snh[s];
-            int rb = find_sorted(h->rows.p, h->rows.n, ql);
-            if (rb < 0 && sl > bad_slot)
-                bad_slot = sl;
-            g_sn[sl] = s;
-            g_rb[sl] = rb | (qe == qlo ? 0 : ASAM_TR_FLAG);
-            g_cb[sl] = qe - pl->desc[s].first;
-        }
-        if (bad_slot >= 0) {
-            asam_set_error("plan: Hessian block (%d,%d) not in the structure of supernode %d", plo.p[bad_slot], phi.p[bad_slot],
-                           g_sn[bad_slot]);
-            free(g_sn);
-            free(g_rb);
-            free(g_cb);
-            return 1;
-        }
-        for (int sl = 0; sl < S; sl++) {
-            sn_host_t *h = &pl->snh[g_sn[sl]];
-            ivec_push(&h->a_slot, sl);
-            ivec_push(&h->a_rb, g_rb[sl]);
-            ivec_push(&h->a_cb, g_cb[sl]);
-        }
-        free(g_sn);
-        free(g_rb);
-        free(g_cb);
-    }
-    ivec_free(&plo);
-    ivec_free(&phi);
-
-    BUILD_LAP(5); /* gather lists */
-    /* 9. layout + schedule */
-    ivec_t seg = { 0 };
-    pl->arena_n = 0;
+    int rel_bad = 0, n_levels = 0;
+#pragma omp parallel for schedule(static, 256) reduction(| : rel_bad) reduction(max : n_levels) if (pl->nsn >= PLAN_OMP_MIN_SN) num_threads(asam_host_threads())
     for (int s = 0; s < pl->nsn; s++) {
-        emit_segment(pl, s, &seg, 0);
-        pl->desc[s].f_off = pl->arena_n;
-        pl->desc[s].reserved = front_doubles(pl->desc[s].mb); /* capacity of this allocation */
-        pl->arena_n += pl->desc[s].reserved;
+        rel_bad |= compute_rel(pl, s);
+        if (pl->desc[s].level + 1 > n_levels)
+            n_levels = pl->desc[s].level + 1;
     }
-    pl->ipool_n = seg.n;
+    pl->n_levels = n_levels;
+    return rel_bad;
+}
 
-    build_schedule(pl);
-
-    BUILD_LAP(6); /* segments + schedule */
-    /* host mirror of the device int pool (debug / tests) */
-    ivec_free(&pl->ipool_host);
-    ivec_reserve(&pl->ipool_host, seg.n);
-    memcpy(pl->ipool_host.p, seg.p, sizeof(int) * (size_t) seg.n);
-    pl->ipool_host.n = seg.n;
-    if (!dev) {
-        ivec_free(&seg);
-        return 0;
+/* Hessian gather lists: the searches in parallel, the lists filled in slot order */
+static int gather_lists(plan_t *pl, const ivec_t *plo, const ivec_t *phi)
+{
+    const int S = pl->n_slots;
+    int *g_sn = malloc(sizeof(int) * (size_t) (S + 1)), *g_rb = malloc(sizeof(int) * (size_t) (S + 1)),
+        *g_cb = malloc(sizeof(int) * (size_t) (S + 1));
+    int bad_slot = -1;
+#pragma omp parallel for schedule(static, 4096) reduction(max : bad_slot) if (S >= 8 * PLAN_OMP_MIN_SN) num_threads(asam_host_threads())
+    for (int sl = 0; sl < S; sl++) {
+        g_sn[sl] = gather_find(pl, plo->p[sl], phi->p[sl], &g_rb[sl], &g_cb[sl]);
+        if (g_rb[sl] < 0 && sl > bad_slot)
+            bad_slot = sl;
     }
+    if (bad_slot >= 0)
+        asam_set_error("plan: Hessian block (%d,%d) not in the structure of supernode %d", plo->p[bad_slot],
+                       phi->p[bad_slot], g_sn[bad_slot]);
+    else
+        for (int sl = 0; sl < S; sl++)
+            gather_push(pl, g_sn[sl], sl, g_rb[sl], g_cb[sl]);
+    free(g_sn); free(g_rb); free(g_cb);
+    return bad_slot >= 0;
+}
 
-    /* 10. upload */
+/* Index segments (into the host copy of the int pool) and arena places of every supernode, in id order */
+static void layout(plan_t *pl)
+{
+    for (int s = 0; s < pl->nsn; s++) {
+        emit_segment(pl, s, &pl->ipool_host, 0);
+        front_place(pl, s, pl->desc[s].mb);
+    }
+    pl->ipool_n = pl->ipool_host.n;
+}
+
+/* Device buffers for the plan, with head-room for incremental steps, and the whole plan uploaded */
+static int build_upload(plan_t *pl, asam_dev_t *dev)
+{
+    const int N = pl->N, n_factors = pl->n_factors, S = pl->n_slots;
     int64_t ipool_cap = pl->ipool_n * 2 + 4096, arena_cap = pl->arena_n + pl->arena_n / 2 + 65536;
     int rc = asam_reserve(dev, N + N / 2 + 64, n_factors + n_factors / 2 + 64, S + S / 2 + 64,
                           pl->nsn + N / 2 + 64, ipool_cap, arena_cap);
@@ -1433,7 +1441,7 @@ static int plan_build_impl(plan_t *pl, asam_dev_t *dev, int N, int n_factors, co
     int *ids = malloc(sizeof(int) * (size_t) pl->nsn);
     for (int s = 0; s < pl->nsn; s++)
         ids[s] = s;
-    rc |= asam_upload_ipool(dev, 0, seg.n, seg.p);
+    rc |= asam_upload_ipool(dev, 0, pl->ipool_host.n, pl->ipool_host.p);
     rc |= asam_upload_desc(dev, pl->nsn, ids, pl->desc);
     rc |= asam_upload_node2q(dev, 0, N, pl->node2q);
     rc |= asam_upload_q2node(dev, 0, N, pl->q2node);
@@ -1441,26 +1449,59 @@ static int plan_build_impl(plan_t *pl, asam_dev_t *dev, int N, int n_factors, co
     rc |= asam_set_full_tasks(dev, pl->ntasks, pl->tasks, pl->nwait, pl->n_btasks, pl->btasks);
     rc |= asam_set_leaf_tasks(dev, pl->n_leaf, pl->leaf_tasks);
     rc |= asam_set_bs_leaf_count(dev, pl->n_bs_leaf);
-    if (pl->world > 1) {
-        asam_shard_sched_t sh;
-        memset(&sh, 0, sizeof(sh));
-        sh.n_top = pl->n_top;
-        sh.top_tasks = pl->top_tasks;
-        sh.top_nwait = pl->top_nwait;
-        sh.n_top_sn = pl->n_top_sn;
-        sh.n_shards = pl->n_shards;
-        sh.shard_owner = pl->shard_owner;
-        sh.shard_off = pl->shard_off;
-        sh.shard_cnt = pl->shard_cnt;
-        sh.shard_q0 = pl->shard_q0;
-        sh.shard_qn = pl->shard_qn;
-        rc |= asam_set_shard_schedule(dev, &sh);
-    } else {
-        rc |= asam_set_shard_schedule(dev, NULL);
-    }
+    asam_shard_sched_t sh = { .n_top = pl->n_top, .top_tasks = pl->top_tasks, .top_nwait = pl->top_nwait,
+                              .n_top_sn = pl->n_top_sn, .n_shards = pl->n_shards, .shard_owner = pl->shard_owner,
+                              .shard_off = pl->shard_off, .shard_cnt = pl->shard_cnt, .shard_q0 = pl->shard_q0,
+                              .shard_qn = pl->shard_qn };
+    rc |= asam_set_shard_schedule(dev, pl->world > 1 ? &sh : NULL);
     free(ids);
-    ivec_free(&seg);
-    BUILD_LAP(7); /* upload */
+    return rc;
+}
+
+static int plan_build_impl(plan_t *pl, asam_dev_t *dev, int N, int n_factors, const int *ftype, const int *fa,
+                           const int *fb, const int *order_keep, int N_keep)
+{
+    plan_reset(pl, dev);
+    if (N <= 0)
+        return 0;
+    int rc = check_factors(0, n_factors, N, 0, ftype, fa, fb);
+    if (rc)
+        return rc;
+    node_arrays_reserve(pl, N);
+    pl->N = N;
+    pl->n_factors = n_factors;
+    double t = pp_now();
+    ivec_t plo = { 0 }, phi = { 0 }; /* pose pairs of the Hessian slots */
+    int *adj_ptr, *adj;
+    pairmap_init(&pl->pairs, n_factors);
+    assign_slots(pl, 0, n_factors, ftype, fa, fb, &plo, &phi);
+    adjacency(N, &plo, &phi, &adj_ptr, &adj);
+    build_lap(0, &t);
+    elimination_order(pl, adj_ptr, adj, order_keep, N_keep);
+    build_lap(1, &t);
+    etree_t et = block_symbolic(pl, adj_ptr, adj);
+    free(adj_ptr); free(adj);
+    build_lap(2, &t);
+    post_order(pl, &et);
+    free(et.head); free(et.next);
+    supernodes(pl, &et);
+    build_lap(3, &t);
+    rc = sn_structure(pl, &et);
+    free(et.bptr); ivec_free(&et.bl); free(et.qpos); free(et.pofq);
+    build_lap(4, &t);
+    if (rc == 0)
+        rc = gather_lists(pl, &plo, &phi);
+    ivec_free(&plo); ivec_free(&phi);
+    if (rc)
+        return rc;
+    build_lap(5, &t);
+    layout(pl);
+    build_schedule(pl);
+    build_lap(6, &t);
+    if (dev) {
+        rc = build_upload(pl, dev);
+        build_lap(7, &t);
+    }
     return rc;
 }
 
@@ -1480,215 +1521,178 @@ int plan_build_with_order(plan_t *pl, asam_dev_t *dev, int N, int n_factors, con
 }
 
 /* ---- incremental append ------------------------------------------------------------------- */
-int plan_append(plan_t *pl, asam_dev_t *dev, int N, int n_factors, const int *ftype, const int *fa, const int *fb,
-                const int *marked_old, int n_marked, int **tasks_out, int **nwait_out, int **keep_out, int *ntasks_out)
-{
-    const int N0 = pl->N, F0 = pl->n_factors, nsn0 = pl->nsn;
-    double pp_t0 = pp_now();
-    *tasks_out = *nwait_out = NULL;
-    if (keep_out)
-        *keep_out = NULL;
-    *ntasks_out = 0;
-    for (int f = F0; f < n_factors; f++) {
-        if (asam_two_pose_type(ftype[f])) {
-            if (fa[f] == fb[f] || fa[f] < 0 || fb[f] < 0 || fa[f] >= N || fb[f] >= N) {
-                asam_set_error("factor %d: bad node ids (%d,%d)", f, fa[f], fb[f]);
-                return 1;
-            }
-            if (fa[f] < N0 && fb[f] < N0)
-                return 2; /* edge between two old poses: structure of old rows changes */
-        } else if (ftype[f] == APRIL_GRAPH_FACTOR_XYTPOS_TYPE) {
-            if (fa[f] < 0 || fa[f] >= N) {
-                asam_set_error("factor %d: bad node id %d", f, fa[f]);
-                return 1;
-            }
-        } else {
-            asam_set_error("factor %d: unsupported factor type %d", f, ftype[f]);
-            return 1;
-        }
-    }
+/* One plan_append step: what its stages hand on.  pl->mark_idx (supernode -> index among the re-factored ones) is -1
+ * between steps; a step sets it for the marked and the created supernodes only, and step_free() resets those. */
+typedef struct {
+    int N0, F0, nsn0, nnew, slot0; /* the plan before the step; new poses; first new Hessian slot */
+    ivec_t nlo, nhi;        /* pose pairs of the new slots slot0, slot0 + 1, ... */
+    int *msn, nm;           /* marked supernodes, ascending id (= children first) */
+    ivec_t *gain;           /* per marked supernode: the new poses it gains as rows */
+    ivec_t *pend, *nbelow;  /* per new pose: children of its supernode, its rows below */
+    int ncreated;           /* supernodes created (ids nsn0, nsn0 + 1, ...) */
+    int bs_leaf_broken;     /* a supernode outgrew k_backsolve_leaf: all go through k_backsolve from now on */
+    int *tasks, *nwait, *keep, nt; /* the fronts to re-factor (keep: their keep words) */
+} step_t;
 
-    if (pl->world > 1) {
-        asam_set_error("a batch solve sharded over %d GPUs cannot be continued incrementally (replicas only)", pl->world);
-        return 1;
+static void step_free(plan_t *pl, step_t *st)
+{
+    for (int i = 0; i < st->nm; i++) {
+        pl->mark_idx[st->msn[i]] = -1;
+        ivec_free(&st->gain[i]);
     }
-    /* incremental steps grow supernodes: the per-block entries of the batch schedule's back-solve list are
-     * replaced by one entry per supernode (parents first = descending id) once, at the first append */
+    for (int k = 0; k < st->ncreated; k++)
+        pl->mark_idx[st->nsn0 + k] = -1;
+    for (int j = 0; st->pend && j < st->nnew; j++) {
+        ivec_free(&st->pend[j]);
+        ivec_free(&st->nbelow[j]);
+    }
+    free(st->gain); free(st->pend); free(st->nbelow); free(st->msn);
+    free(st->tasks); free(st->nwait); free(st->keep);
+    ivec_free(&st->nlo); ivec_free(&st->nhi);
+}
+
+/* Incremental steps grow supernodes and run the whole schedule through k_factor / k_backsolve: at the first append the
+ * batch back-solve list gets one entry per supernode (parents first = descending id), and the leaf launches go. */
+static int step_form(plan_t *pl, asam_dev_t *dev)
+{
+    const int nsn = pl->nsn;
     if (pl->bt_split) {
-        int *plain = malloc(sizeof(int) * (size_t) (nsn0 + 1));
-        for (int sx = 0; sx < nsn0; sx++)
-            plain[sx] = nsn0 - 1 - sx;
+        int *plain = malloc(sizeof(int) * (size_t) (nsn + 1));
+        for (int sx = 0; sx < nsn; sx++)
+            plain[sx] = nsn - 1 - sx;
         free(pl->btasks);
         pl->btasks = plain;
-        pl->n_btasks = nsn0;
+        pl->n_btasks = nsn;
         pl->bt_split = 0;
         pl->n_bs_leaf = 0;
         if (dev && (asam_set_full_tasks(dev, pl->ntasks, pl->tasks, pl->nwait, pl->n_btasks, pl->btasks) ||
                     asam_set_bs_leaf_count(dev, 0)))
             return 1;
     }
-    /* incremental steps run the whole schedule through k_factor / k_backsolve */
     if (pl->n_leaf > 0) {
         pl->n_leaf = 0;
         if (dev && asam_set_leaf_tasks(dev, 0, NULL))
             return 1;
     }
+    return 0;
+}
 
-    /* grow node-indexed arrays: new poses are eliminated last, in id order */
+/* Node-indexed arrays for N poses and room for a supernode per new pose: new poses are eliminated last, in id order */
+static void grow_arrays(plan_t *pl, int N, const step_t *st)
+{
     node_arrays_reserve(pl, N);
-    fslot_reserve(pl, n_factors);
-    const int nnew = N - N0;
-    sn_arrays_reserve(pl, nsn0 + nnew);
-    for (int i = N0; i < N; i++) {
-        pl->order[i] = i;
-        pl->pos[i] = i;
-        pl->node2q[i] = i;
-        pl->q2node[i] = i;
-        pl->parent_pos[i] = -1;
-        pl->sn_of_q[i] = -1; /* assigned below: joins the root supernode or gets a new one */
+    sn_arrays_reserve(pl, st->nsn0 + st->nnew);
+    for (int i = st->N0; i < N; i++) {
+        pl->order[i] = pl->pos[i] = pl->node2q[i] = pl->q2node[i] = i;
+        pl->parent_pos[i] = pl->sn_of_q[i] = -1; /* sn_of_q: set by place_new_poses() */
     }
+}
 
-    /* new Hessian slots */
-    const int slot0 = pl->n_slots;
-    ivec_t nlo = { 0 }, nhi = { 0 };
-    for (int f = F0; f < n_factors; f++) {
-        if (!asam_two_pose_type(ftype[f])) {
-            pl->fslot[f] = -1;
-            continue;
-        }
-        int a = fa[f], b = fb[f], lo = a < b ? a : b, hi = a < b ? b : a, created;
-        int slot = pairmap_get_or_add(&pl->pairs, lo, hi, pl->n_slots, &created);
-        if (created) {
-            ivec_push(&nlo, lo);
-            ivec_push(&nhi, hi);
-            pl->n_slots++;
-        }
-        pl->fslot[f] = slot;
-    }
-
-    /* marked supernodes, ascending id (= children first) */
-    int *msn = malloc(sizeof(int) * (size_t) (n_marked + 1));
-    int nm = 0;
+/* The marked supernodes, their mark_idx and their keep words.  Partial re-factorisation: the columns of a marked
+ * supernode BEFORE its first marked pose are unchanged by this step (their Hessian entries, their children and --
+ * because a new pose reaches an old column only through a marked one -- their rows), so the kernel keeps them (L and
+ * y) and re-eliminates from the first marked column on: keep[i] = (poses kept << 16) | block rows before this step
+ * (the retained front still has that layout), 0 = re-factor the whole front. */
+static void mark_supernodes(plan_t *pl, step_t *st, const int *marked_old, int n_marked)
+{
+    st->msn = malloc(sizeof(int) * (size_t) (n_marked + 1));
     for (int i = 0; i < n_marked; i++)
-        if (marked_old[i] < N0)
-            msn[nm++] = pl->sn_of_q[pl->node2q[marked_old[i]]];
-    nm = sort_unique(msn, nm);
-    /* sn -> index in msn or -1: kept across steps, all -1 between them (an O(nsn) fill per step is what made the
-     * reference's incremental steps grow with the graph, SURVEY.md quirk 13) */
+        if (marked_old[i] < st->N0)
+            st->msn[st->nm++] = pl->sn_of_q[pl->node2q[marked_old[i]]];
+    st->nm = sort_unique(st->msn, st->nm);
+    /* mark_idx is kept across steps, all -1 between them (an O(nsn) fill per step is what made the reference's
+     * incremental steps grow with the graph, SURVEY.md quirk 13) */
     if (pl->sn_cap > pl->mark_cap) {
         pl->mark_idx = realloc(pl->mark_idx, sizeof(int) * (size_t) pl->sn_cap);
         for (int s = pl->mark_cap; s < pl->sn_cap; s++)
             pl->mark_idx[s] = -1;
         pl->mark_cap = pl->sn_cap;
     }
-    int *mark_idx = pl->mark_idx;
-    for (int i = 0; i < nm; i++)
-        mark_idx[msn[i]] = i;
-
-    /* Partial re-factorisation: the columns of a marked supernode BEFORE its first marked pose are
-     * unchanged by this step (their Hessian entries, their children and -- because a new pose reaches an
-     * old column only through a marked one -- their rows), so the kernel keeps them (L and y) and
-     * re-eliminates from the first marked column on.  keepb[i] = poses kept of marked supernode i,
-     * oldmb[i] = its block rows before this step (the retained front still has that layout). */
-    int *keepb = malloc(sizeof(int) * (size_t) (nm + 1)), *oldmb = malloc(sizeof(int) * (size_t) (nm + 1));
-    for (int i = 0; i < nm; i++) {
-        keepb[i] = pl->desc[msn[i]].cb;
-        oldmb[i] = pl->snh[msn[i]].rows.n;
-    }
+    for (int i = 0; i < st->nm; i++)
+        pl->mark_idx[st->msn[i]] = i;
+    st->gain = calloc((size_t) st->nm + 1, sizeof(ivec_t));
+    st->keep = calloc((size_t) (st->nm + st->nnew) + 1, sizeof(int)); /* (created supernodes: 0) */
+    for (int i = 0; i < st->nm; i++)
+        st->keep[i] = pl->desc[st->msn[i]].cb;
     for (int i = 0; i < n_marked; i++)
-        if (marked_old[i] < N0) {
-            int q = pl->node2q[marked_old[i]], sidx = mark_idx[pl->sn_of_q[q]];
-            int k = q - pl->desc[msn[sidx]].first;
-            if (k < keepb[sidx])
-                keepb[sidx] = k;
+        if (marked_old[i] < st->N0) {
+            int q = pl->node2q[marked_old[i]], sidx = pl->mark_idx[pl->sn_of_q[q]];
+            int k = q - pl->desc[st->msn[sidx]].first;
+            if (k < st->keep[sidx])
+                st->keep[sidx] = k;
         }
+    for (int i = 0; i < st->nm; i++) {
+        const int kept = st->keep[i], oldmb = pl->snh[st->msn[i]].rows.n;
+        st->keep[i] = kept > 0 && kept < 0x7fff && oldmb < 0xffff ? (kept << 16) | oldmb : 0;
+    }
+}
 
-    int rc = 0, bs_leaf_broken = 0;
-    ivec_t *gain = calloc((size_t) nm + 1, sizeof(ivec_t));
-    ivec_t *pend = calloc((size_t) nnew + 1, sizeof(ivec_t)); /* children of each new supernode */
-    ivec_t *nbelow = calloc((size_t) nnew + 1, sizeof(ivec_t));
-
-    /* seed gains with the new edges (old pose, new pose); new-new edges seed nbelow */
-    for (int k = 0; k < nlo.n; k++) {
-        int lo = nlo.p[k], hi = nhi.p[k];
+/* The new poses that become rows of the marked supernodes: those of their new (old, new) blocks, and, up the marked
+ * sub-forest, those of their marked children.  A front that outgrows its allocation moves; an old root hangs under
+ * the first new pose it gains.  The (new, new) blocks seed the rows below the new poses. */
+static int propagate_gains(plan_t *pl, step_t *st)
+{
+    const int N0 = st->N0;
+    int *mark_idx = pl->mark_idx;
+    st->pend = calloc((size_t) st->nnew + 1, sizeof(ivec_t));
+    st->nbelow = calloc((size_t) st->nnew + 1, sizeof(ivec_t));
+    for (int k = 0; k < st->nlo.n; k++) {
+        int lo = st->nlo.p[k], hi = st->nhi.p[k];
         if (lo < N0) {
             int s = pl->sn_of_q[pl->node2q[lo]];
             if (mark_idx[s] < 0) {
                 asam_set_error("plan_append: pose %d gets a new factor but is not marked", lo);
-                rc = 1;
-                goto done;
+                return 1;
             }
-            ivec_push(&gain[mark_idx[s]], hi);
+            ivec_push(&st->gain[mark_idx[s]], hi);
         } else {
-            ivec_push(&nbelow[lo - N0], hi);
+            ivec_push(&st->nbelow[lo - N0], hi);
         }
     }
-
-    /* propagate gains up the marked sub-forest; grow row lists; re-place fronts */
-    for (int i = 0; i < nm; i++) {
-        int s = msn[i];
+    for (int i = 0; i < st->nm; i++) {
+        int s = st->msn[i];
         sn_host_t *h = &pl->snh[s];
         asam_sn_desc_t *d = &pl->desc[s];
+        ivec_t *gain = &st->gain[i];
         for (int c = 0; c < h->children.n; c++) {
             int ci = mark_idx[h->children.p[c]];
             if (ci >= 0)
-                for (int e = 0; e < gain[ci].n; e++)
-                    ivec_push(&gain[i], gain[ci].p[e]);
+                for (int e = 0; e < st->gain[ci].n; e++)
+                    ivec_push(gain, st->gain[ci].p[e]);
         }
-        gain[i].n = sort_unique(gain[i].p, gain[i].n);
+        gain->n = sort_unique(gain->p, gain->n);
         int old_mb = h->rows.n;
-        for (int e = 0; e < gain[i].n; e++)
-            ivec_push(&h->rows, gain[i].p[e]); /* new poses sort after every old row */
-        d->mb = h->rows.n;
-        if (3 * d->mb > pl->max_m)
-            pl->max_m = 3 * d->mb;
-        if (pl->n_bs_leaf > 0 && pl->bs_leaf[s] && 3 * (d->mb - d->cb) > ASAM_BSLEAF_MAX)
-            bs_leaf_broken = 1; /* outgrew the warp kernel: everything goes through k_backsolve from now on */
+        for (int e = 0; e < gain->n; e++)
+            ivec_push(&h->rows, gain->p[e]); /* new poses sort after every old row */
+        sn_set_mb(pl, s);
+        st->bs_leaf_broken |= bs_leaf_outgrown(pl, s);
         if (d->mb != old_mb && front_doubles(d->mb) > d->reserved) {
             /* the front outgrew its allocation: move it, with head-room for the poses that
              * later steps will append (the old space is reclaimed at the next batch) */
-            int slack = d->mb / 4 > 4 ? d->mb / 4 : 4;
-            d->reserved = front_doubles(d->mb + slack);
-            d->f_off = pl->arena_n;
-            pl->arena_n += d->reserved;
-            keepb[i] = 0; /* the retained columns stay behind at the old place */
+            front_place(pl, s, d->mb + (d->mb / 4 > 4 ? d->mb / 4 : 4));
+            st->keep[i] = 0; /* the retained columns stay behind at the old place */
         }
-        if (d->parent < 0 && gain[i].n > 0) { /* old root: hangs under the first new pose */
-            ivec_push(&pend[gain[i].p[0] - N0], s); /* supernode id of that pose: set below */
+        if (d->parent < 0 && gain->n > 0) { /* old root: hangs under the first new pose */
+            ivec_push(&st->pend[gain->p[0] - N0], s); /* supernode id of that pose: set by place_new_poses() */
             int top = pl->q2node[d->first + d->cb - 1];
-            pl->parent_pos[pl->pos[top]] = gain[i].p[0]; /* pos == q == id for new poses */
+            pl->parent_pos[pl->pos[top]] = gain->p[0]; /* pos == q == id for new poses */
         }
     }
-    /* gather-list entries for the new (old,new) blocks */
-    for (int k = 0; k < nlo.n; k++) {
-        int lo = nlo.p[k], hi = nhi.p[k];
-        if (lo >= N0)
-            continue;
-        int s = pl->sn_of_q[pl->node2q[lo]];
-        sn_host_t *h = &pl->snh[s];
-        int rb = find_sorted(h->rows.p, h->rows.n, hi);
-        if (rb < 0) {
-            asam_set_error("plan_append: internal (row %d not in supernode %d)", hi, s);
-            rc = 1;
-            goto done;
-        }
-        ivec_push(&h->a_slot, slot0 + k);
-        ivec_push(&h->a_rb, rb); /* early = lo = lower id: no transpose */
-        ivec_push(&h->a_cb, pl->node2q[lo] - pl->desc[s].first);
-    }
+    return 0;
+}
 
-    /* new poses, ascending.  A pose whose predecessor in the order tops a root supernode with
-     * exactly the structure {pose} + below(pose) becomes one more COLUMN of that supernode
-     * (fundamental merge) -- otherwise every step would add one more link to the chain at the top
-     * of the tree; any other pose starts a singleton supernode. */
-    int *nsid = malloc(sizeof(int) * (size_t) (nnew + 1));
-    int ncreated = 0;
-    for (int j = 0; j < nnew; j++) {
+/* New poses, ascending.  A pose whose predecessor in the order tops a root supernode with exactly the structure
+ * {pose} + below(pose) becomes one more COLUMN of that supernode (fundamental merge) -- otherwise every step would add
+ * one more link to the chain at the top of the tree; any other pose starts a singleton supernode. */
+static void place_new_poses(plan_t *pl, step_t *st)
+{
+    const int N0 = st->N0;
+    for (int j = 0; j < st->nnew; j++) {
         int n = N0 + j;
-        ivec_t *bel = &nbelow[j];
+        ivec_t *bel = &st->nbelow[j], *pend = &st->pend[j];
         int lvl = 0;
-        for (int c = 0; c < pend[j].n; c++) {
-            int X = pend[j].p[c];
+        for (int c = 0; c < pend->n; c++) {
+            int X = pend->p[c];
             const sn_host_t *hx = &pl->snh[X];
             for (int e = pl->desc[X].cb; e < hx->rows.n; e++)
                 if (hx->rows.p[e] != n)
@@ -1700,218 +1704,213 @@ int plan_append(plan_t *pl, asam_dev_t *dev, int N, int n_factors, const int *ft
         int R = n > 0 ? pl->sn_of_q[n - 1] : -1, sid = -1;
         if (R >= 0 && pl->desc[R].cb < MAX_SN_COLS && pl->desc[R].first + pl->desc[R].cb == n &&
             pl->snh[R].rows.n - pl->desc[R].cb == 1 + bel->n) {
-            for (int c = 0; c < pend[j].n; c++)
-                if (pend[j].p[c] == R)
+            for (int c = 0; c < pend->n; c++)
+                if (pend->p[c] == R)
                     sid = R;
         }
         if (sid >= 0) { /* n joins R: the row list already holds n right after R's columns */
             asam_sn_desc_t *d = &pl->desc[R];
-            sn_host_t *h = &pl->snh[R];
             d->cb += 1;
-            if (pl->n_bs_leaf > 0 && pl->bs_leaf[R] && 3 * d->cb > ASAM_BSLEAF_MAX)
-                bs_leaf_broken = 1;
-            for (int c = 0; c < pend[j].n; c++) {
-                int X = pend[j].p[c];
+            st->bs_leaf_broken |= bs_leaf_outgrown(pl, R);
+            for (int c = 0; c < pend->n; c++) {
+                int X = pend->p[c];
                 if (X == R)
                     continue;
-                ivec_push(&h->children, X);
+                ivec_push(&pl->snh[R].children, X);
                 pl->desc[X].parent = R;
             }
             if (lvl > d->level)
                 d->level = lvl;
             d->parent = -1;
         } else {
-            sid = pl->nsn++;
-            ncreated++;
-            asam_sn_desc_t *d = &pl->desc[sid];
+            sid = sn_create(pl, n);
+            st->ncreated++;
             sn_host_t *h = &pl->snh[sid];
-            memset(d, 0, sizeof(*d));
-            d->first = n;
-            d->cb = 1;
-            d->parent = -1;
-            d->level = lvl;
-            h->rows.n = 0;
+            pl->desc[sid].level = lvl;
             ivec_push(&h->rows, n);
             for (int e = 0; e < bel->n; e++)
                 ivec_push(&h->rows, bel->p[e]);
-            h->children.n = 0;
-            for (int c = 0; c < pend[j].n; c++) {
-                ivec_push(&h->children, pend[j].p[c]);
-                pl->desc[pend[j].p[c]].parent = sid;
+            for (int c = 0; c < pend->n; c++) {
+                ivec_push(&h->children, pend->p[c]);
+                pl->desc[pend->p[c]].parent = sid;
             }
-            h->a_slot.n = h->a_rb.n = h->a_cb.n = 0;
-            d->mb = h->rows.n;
-            if (3 * d->mb > pl->max_m)
-                pl->max_m = 3 * d->mb;
-            d->reserved = front_doubles(d->mb + 4);
-            d->f_off = pl->arena_n;
-            pl->arena_n += d->reserved;
+            sn_set_mb(pl, sid);
+            front_place(pl, sid, pl->desc[sid].mb + 4);
         }
-        nsid[j] = sid;
         pl->sn_of_q[n] = sid;
         if (bel->n > 0) {
-            ivec_push(&pend[bel->p[0] - N0], sid);
+            ivec_push(&st->pend[bel->p[0] - N0], sid);
             pl->parent_pos[n] = bel->p[0];
         }
         if (pl->desc[sid].level + 1 > pl->n_levels)
             pl->n_levels = pl->desc[sid].level + 1;
     }
-    for (int k = 0; k < nlo.n; k++) { /* (new,new) blocks */
-        int lo = nlo.p[k], hi = nhi.p[k];
-        if (lo < N0)
-            continue;
-        int s = nsid[lo - N0];
-        sn_host_t *h = &pl->snh[s];
-        int rb = find_sorted(h->rows.p, h->rows.n, hi);
-        if (rb < 0) {
-            asam_set_error("plan_append: internal (row %d not in new supernode %d)", hi, s);
+}
+
+/* Gather entries of the new slots: the (old, new) blocks, then the (new, new) ones */
+static int gather_entries(plan_t *pl, const step_t *st)
+{
+    for (int pass = 0; pass < 2; pass++)
+        for (int k = 0; k < st->nlo.n; k++) {
+            int lo = st->nlo.p[k], hi = st->nhi.p[k], rb, cb;
+            if ((lo >= st->N0) != pass)
+                continue;
+            int s = gather_find(pl, lo, hi, &rb, &cb);
+            if (rb < 0) {
+                asam_set_error("plan_append: internal (row %d not in %ssupernode %d)", hi, pass ? "new " : "", s);
+                return 1;
+            }
+            gather_push(pl, s, st->slot0 + k, rb, cb);
+        }
+    return 0;
+}
+
+/* The fronts to re-factor, marked then created, with their child counts, relative indices and index segments
+ * (appended to the host copy of the int pool); every new pose must be in one of them */
+static int step_fronts(plan_t *pl, step_t *st)
+{
+    int rc = 0;
+    st->nt = st->nm + st->ncreated;
+    st->tasks = malloc(sizeof(int) * (size_t) (st->nt + 1));
+    st->nwait = malloc(sizeof(int) * (size_t) (st->nt + 1));
+    memcpy(st->tasks, st->msn, sizeof(int) * (size_t) st->nm);
+    for (int k = 0; k < st->ncreated; k++) {
+        st->tasks[st->nm + k] = st->nsn0 + k;
+        pl->mark_idx[st->nsn0 + k] = st->nm + k;
+    }
+    for (int n = st->N0; n < st->N0 + st->nnew; n++) /* a pose may have joined a supernode that was not marked */
+        if (pl->mark_idx[pl->sn_of_q[n]] < 0) {
+            asam_set_error("plan_append: pose %d joined unmarked supernode %d", n, pl->sn_of_q[n]);
             rc = 1;
-            free(nsid);
-            goto done;
         }
-        ivec_push(&h->a_slot, slot0 + k);
-        ivec_push(&h->a_rb, rb);
-        ivec_push(&h->a_cb, lo - pl->desc[s].first);
+    for (int t = 0; t < st->nt && !rc; t++)
+        rc = compute_rel(pl, st->tasks[t]);
+    for (int t = 0; t < st->nt && !rc; t++) {
+        int s = st->tasks[t], w = 0;
+        for (int c = 0; c < pl->snh[s].children.n; c++)
+            if (pl->mark_idx[pl->snh[s].children.p[c]] >= 0)
+                w++;
+        st->nwait[t] = pack_nwait(w, 0, 0);
+        emit_segment(pl, s, &pl->ipool_host, 0); /* the host pool holds pl->ipool_n ints before the step */
     }
+    return rc;
+}
 
-    /* relative indices + segments of everything that changed */
-    {
-        int nt = nm + ncreated;
-        int *tasks = malloc(sizeof(int) * (size_t) (nt + 1)), *nwait = malloc(sizeof(int) * (size_t) (nt + 1));
-        int *keep = calloc((size_t) nt + 1, sizeof(int));
-        for (int i = 0; i < nm; i++) {
-            tasks[i] = msn[i];
-            if (keepb[i] > 0 && keepb[i] < 0x7fff && oldmb[i] < 0xffff)
-                keep[i] = (keepb[i] << 16) | oldmb[i];
-        }
-        for (int k = 0; k < ncreated; k++) { /* created supernodes have ids nsn0 .. nsn0+ncreated-1 */
-            tasks[nm + k] = nsn0 + k;
-            mark_idx[nsn0 + k] = nm + k;
-        }
-        for (int j = 0; j < nnew; j++) /* a pose may have joined a supernode that was not marked */
-            if (mark_idx[nsid[j]] < 0) {
-                asam_set_error("plan_append: pose %d joined unmarked supernode %d", N0 + j, nsid[j]);
-                rc = 1;
-            }
-        free(nsid);
-        ivec_t seg = { 0 };
-        for (int t = 0; t < nt && !rc; t++)
-            rc |= compute_rel(pl, tasks[t]);
-        for (int t = 0; t < nt && !rc; t++) {
-            int s = tasks[t], w = 0;
-            for (int c = 0; c < pl->snh[s].children.n; c++)
-                if (mark_idx[pl->snh[s].children.p[c]] >= 0)
-                    w++;
-            nwait[t] = pack_nwait(w, 0, 0);
-            emit_segment(pl, s, &seg, pl->ipool_n);
-        }
-        if (!rc) {
-            ivec_reserve(&pl->ipool_host, pl->ipool_host.n + seg.n);
-            memcpy(pl->ipool_host.p + pl->ipool_host.n, seg.p, sizeof(int) * (size_t) seg.n);
-            pl->ipool_host.n += seg.n;
-        }
-        if (!rc && !dev)
-            pl->ipool_n += seg.n;
-        if (!rc && !dev && bs_leaf_broken) /* (with a device: below, together with the device's count) */
+/* What the step changed, to the device: segments and descriptors of the fronts, the new poses, the new supernodes at
+ * the head of the back-solve list (ancestors of all older ones), the new factors' slots; new Hessian entries cleared */
+static int step_upload(plan_t *pl, asam_dev_t *dev, const step_t *st, int N, int n_factors)
+{
+    double t = pp_now();
+    const int nt = st->nt, nnew = st->nnew, ncreated = st->ncreated;
+    const int64_t ipool_need = pl->ipool_host.n;
+    int rc = asam_reserve(dev, N + 64, n_factors + 64, pl->n_slots + 64, pl->nsn + 64, ipool_need + ipool_need / 2,
+                          pl->arena_n + pl->arena_n / 4);
+    g_plan_prof[1] += pp_now() - t; /* asam_reserve */
+    t = pp_now();
+    asam_sn_desc_t *dd = malloc(sizeof(asam_sn_desc_t) * (size_t) (nt + 1));
+    for (int k = 0; k < nt; k++)
+        dd[k] = pl->desc[st->tasks[k]];
+    if (!rc)
+        rc |= asam_upload_ipool(dev, pl->ipool_n, ipool_need - pl->ipool_n, pl->ipool_host.p + pl->ipool_n);
+    if (!rc)
+        rc |= asam_upload_desc(dev, nt, st->tasks, dd);
+    if (!rc && nnew > 0) {
+        rc |= asam_upload_node2q(dev, st->N0, nnew, pl->node2q + st->N0);
+        rc |= asam_upload_q2node(dev, st->N0, nnew, pl->q2node + st->N0);
+    }
+    if (!rc && ncreated > 0) {
+        int *pre = malloc(sizeof(int) * (size_t) ncreated);
+        for (int k = 0; k < ncreated; k++)
+            pre[k] = st->nsn0 + ncreated - 1 - k;
+        rc |= asam_btasks_prepend(dev, ncreated, pre);
+        free(pre);
+    }
+    if (!rc && st->bs_leaf_broken)
+        rc |= asam_set_bs_leaf_count(dev, 0);
+    if (!rc)
+        rc |= asam_upload_fslot(dev, st->F0, n_factors - st->F0, pl->fslot + st->F0);
+    if (!rc)
+        rc |= asam_hessian_clear_range(dev, st->N0, nnew, st->slot0, pl->n_slots - st->slot0);
+    free(dd);
+    g_plan_prof[2] += pp_now() - t; /* uploads */
+    return rc;
+}
+
+/* Fronts that teams factor become consecutive task entries, one per worker (emit_front); teams re-factor whole fronts */
+static void expand_teams(const plan_t *pl, step_t *st)
+{
+    int total = 0;
+    for (int t = 0; t < st->nt; t++)
+        total += front_ctas(team_size(pl->desc[st->tasks[t]].mb, pl->desc[st->tasks[t]].cb, plan_team_cap(pl)));
+    if (total == st->nt)
+        return;
+    int *t2 = malloc(sizeof(int) * (size_t) total), *w2 = malloc(sizeof(int) * (size_t) total);
+    int *k2 = calloc((size_t) total, sizeof(int)), k = 0;
+    for (int t = 0; t < st->nt; t++) {
+        const int G = team_size(pl->desc[st->tasks[t]].mb, pl->desc[st->tasks[t]].cb, plan_team_cap(pl));
+        if (G == 0)
+            k2[k] = st->keep[t];
+        k += emit_front(t2 + k, w2 + k, st->tasks[t], st->nwait[t], G);
+    }
+    free(st->tasks); free(st->nwait); free(st->keep);
+    st->tasks = t2;
+    st->nwait = w2;
+    st->keep = k2;
+    st->nt = total;
+}
+
+int plan_append(plan_t *pl, asam_dev_t *dev, int N, int n_factors, const int *ftype, const int *fa, const int *fb,
+                const int *marked_old, int n_marked, int **tasks_out, int **nwait_out, int **keep_out, int *ntasks_out)
+{
+    const double t0 = pp_now();
+    *tasks_out = *nwait_out = NULL;
+    if (keep_out)
+        *keep_out = NULL;
+    *ntasks_out = 0;
+    step_t st = { .N0 = pl->N, .F0 = pl->n_factors, .nsn0 = pl->nsn, .nnew = N - pl->N };
+    /* everything is checked before anything changes: after a 2 the caller rebuilds from this plan */
+    int rc = check_factors(st.F0, n_factors, N, st.N0, ftype, fa, fb);
+    if (rc == 0 && pl->world > 1) {
+        asam_set_error("a batch solve sharded over %d GPUs cannot be continued incrementally (replicas only)", pl->world);
+        rc = 1;
+    }
+    if (rc == 0)
+        rc = step_form(pl, dev);
+    if (rc == 0) {
+        grow_arrays(pl, N, &st);
+        st.slot0 = pl->n_slots;
+        assign_slots(pl, st.F0, n_factors, ftype, fa, fb, &st.nlo, &st.nhi);
+        mark_supernodes(pl, &st, marked_old, n_marked);
+        rc = propagate_gains(pl, &st);
+    }
+    if (rc == 0) {
+        place_new_poses(pl, &st);
+        rc = gather_entries(pl, &st);
+    }
+    if (rc == 0) {
+        rc = step_fronts(pl, &st);
+        g_plan_prof[0] += pp_now() - t0; /* host symbolic */
+    }
+    if (rc == 0 && dev)
+        rc = step_upload(pl, dev, &st, N, n_factors);
+    if (rc == 0) {
+        pl->ipool_n = pl->ipool_host.n;
+        if (st.bs_leaf_broken)
             pl->n_bs_leaf = 0;
-        g_plan_prof[0] += pp_now() - pp_t0; /* host symbolic */
-        pp_t0 = pp_now();
-        if (!rc && dev) {
-            int64_t ipool_need = pl->ipool_n + seg.n;
-            rc = asam_reserve(dev, N + 64, n_factors + 64, pl->n_slots + 64, pl->nsn + 64, ipool_need + ipool_need / 2,
-                              pl->arena_n + pl->arena_n / 4);
-            g_plan_prof[1] += pp_now() - pp_t0; /* asam_reserve */
-            pp_t0 = pp_now();
-            asam_sn_desc_t *dd = malloc(sizeof(asam_sn_desc_t) * (size_t) (nt + 1));
-            for (int t = 0; t < nt; t++)
-                dd[t] = pl->desc[tasks[t]];
-            if (!rc)
-                rc |= asam_upload_ipool(dev, pl->ipool_n, seg.n, seg.p);
-            if (!rc)
-                rc |= asam_upload_desc(dev, nt, tasks, dd);
-            if (!rc && nnew > 0) {
-                rc |= asam_upload_node2q(dev, N0, nnew, pl->node2q + N0);
-                rc |= asam_upload_q2node(dev, N0, nnew, pl->q2node + N0);
-            }
-            if (!rc && ncreated > 0) { /* new supernodes are ancestors of all older ones */
-                int *pre = malloc(sizeof(int) * (size_t) ncreated);
-                for (int k = 0; k < ncreated; k++)
-                    pre[k] = nsn0 + ncreated - 1 - k;
-                rc |= asam_btasks_prepend(dev, ncreated, pre);
-                free(pre);
-            }
-            if (!rc && bs_leaf_broken) {
-                pl->n_bs_leaf = 0;
-                rc |= asam_set_bs_leaf_count(dev, 0);
-            }
-            if (!rc)
-                rc |= asam_upload_fslot(dev, F0, n_factors - F0, pl->fslot + F0);
-            if (!rc)
-                rc |= asam_hessian_clear_range(dev, N0, nnew, slot0, pl->n_slots - slot0);
-            free(dd);
-            pl->ipool_n += seg.n;
-            g_plan_prof[2] += pp_now() - pp_t0; /* uploads */
+        expand_teams(pl, &st);
+        *tasks_out = st.tasks;
+        *nwait_out = st.nwait;
+        *ntasks_out = st.nt;
+        st.tasks = st.nwait = NULL;
+        if (keep_out) {
+            *keep_out = st.keep;
+            st.keep = NULL;
         }
-        ivec_free(&seg);
-        if (rc) {
-            free(tasks);
-            free(nwait);
-            free(keep);
-        } else {
-            /* expand big fronts into teams of consecutive entries */
-            int total = 0;
-            for (int t = 0; t < nt; t++)
-                total += front_ctas(team_size(pl->desc[tasks[t]].mb, pl->desc[tasks[t]].cb, plan_team_cap(pl)));
-            if (total != nt) {
-                int *t2 = malloc(sizeof(int) * (size_t) total), *w2 = malloc(sizeof(int) * (size_t) total);
-                int *k2 = calloc((size_t) total, sizeof(int)); /* teams re-factor whole fronts */
-                int k = 0;
-                for (int t = 0; t < nt; t++) {
-                    const int G = team_size(pl->desc[tasks[t]].mb, pl->desc[tasks[t]].cb, plan_team_cap(pl));
-                    if (G == 0)
-                        k2[k] = keep[t];
-                    k += emit_front(t2 + k, w2 + k, tasks[t], nwait[t], G);
-                }
-                free(tasks);
-                free(nwait);
-                free(keep);
-                tasks = t2;
-                nwait = w2;
-                keep = k2;
-                nt = total;
-            }
-            *tasks_out = tasks;
-            *nwait_out = nwait;
-            if (keep_out)
-                *keep_out = keep;
-            else
-                free(keep);
-            *ntasks_out = nt;
-        }
+        pl->N = N;
+        pl->n_factors = n_factors;
+        pl->struct_hash = 0; /* appended order: never to be reused by a batch solve (it re-orders) */
     }
-    pl->N = N;
-    pl->n_factors = n_factors;
-    pl->struct_hash = 0; /* appended order: never to be reused by a batch solve (it re-orders) */
-
-done:
-    for (int i = 0; i < nm; i++)
-        ivec_free(&gain[i]);
-    for (int j = 0; j < nnew; j++) {
-        ivec_free(&pend[j]);
-        ivec_free(&nbelow[j]);
-    }
-    for (int i = 0; i < nm; i++)
-        mark_idx[msn[i]] = -1;
-    for (int sx = nsn0; sx < nsn0 + nnew && sx < pl->mark_cap; sx++)
-        mark_idx[sx] = -1;
-    free(gain);
-    free(pend);
-    free(nbelow);
-    free(msn);
-    free(keepb);
-    free(oldmb);
-    ivec_free(&nlo);
-    ivec_free(&nhi);
+    step_free(pl, &st);
     return rc;
 }
 
