@@ -102,6 +102,7 @@ struct asam_dev {
     Buf partial;  // chi2 partial sums
     Buf patch_ids, patch_desc;
     Buf pts;
+    Buf rb_int, rb_dbl; // tables of asam_hessian_rebuild
     int epoch = 0;
 
     // host->device traffic is BATCHED: small uploads and fills are queued in one pinned staging
@@ -307,12 +308,13 @@ static int download(asam_dev *d, void *dst, const void *src, size_t bytes)
 #define ASAM_SPIN_LIMIT_NS 20000000000LL
 
 struct Pending {
-    int kind; // 0 linearize, 1 factor, 2 backsolve
+    int kind; // 0 linearize, 1 factor, 2 backsolve, 3 Hessian rebuild
     int grid;
     int nleaf;
     LinArgs lin;
     FacArgs fac;
     BsArgs bs;
+    RebuildArgs rb;
 };
 #define ASAM_MAX_PENDING 8
 
@@ -327,6 +329,15 @@ static int run_linearize(asam_dev *d, const LinArgs &a)
         CK(cudaEventRecord(d->ev[1], d->stream));
         d->ev_set[0] = 1;
     }
+    return 0;
+}
+
+static int run_rebuild(asam_dev *d, const RebuildArgs &a)
+{
+    const int warps = a.n_pose + (a.n_slot + 31) / 32;
+    k_hessian_rebuild<<<(warps + 3) / 4, 128, 0, d->stream>>>(a);
+    d->n_launch++;
+    CK(cudaGetLastError());
     return 0;
 }
 
@@ -425,8 +436,10 @@ ASAM_EXPORT int asam_step_run(asam_dev_t *d)
         return 1;
     for (int i = 0; i < d->npend; i++) {
         Pending &p = d->pend[i];
-        int rc = p.kind == 0 ? run_linearize(d, p.lin) : p.kind == 1 ? run_factor(d, p.fac, p.grid)
-                                                                      : run_backsolve(d, p.bs, p.grid, p.nleaf);
+        int rc = p.kind == 0   ? run_linearize(d, p.lin)
+                 : p.kind == 1 ? run_factor(d, p.fac, p.grid)
+                 : p.kind == 2 ? run_backsolve(d, p.bs, p.grid, p.nleaf)
+                               : run_rebuild(d, p.rb);
         if (rc)
             return rc;
     }
@@ -625,7 +638,7 @@ ASAM_EXPORT void asam_dev_destroy(asam_dev_t *d)
     Buf *all[] = { &d->f_type, &d->f_a, &d->f_b, &d->f_z, &d->f_W, &d->f_slot, &d->f_loss, &d->lp, &d->st, &d->node2q, &d->q2node,
                    &d->Adiag, &d->Aoff, &d->Bq, &d->y, &d->x, &d->dinv, &d->sn, &d->ipool, &d->arena, &d->arrive,
                    &d->xdone, &d->xblk, &d->tbar, &d->tasks_full, &d->nwait_full, &d->btasks_full, &d->tasks_tmp, &d->nwait_tmp,
-                   &d->btasks_tmp, &d->keep_tmp, &d->leaf_tasks, &d->top_tasks, &d->top_nwait, &d->ctrl, &d->partial, &d->patch_ids, &d->patch_desc, &d->pts, &d->flush, &d->trace_fac, &d->trace_bs, &d->ptrace, &d->marg };
+                   &d->btasks_tmp, &d->keep_tmp, &d->leaf_tasks, &d->top_tasks, &d->top_nwait, &d->ctrl, &d->partial, &d->patch_ids, &d->patch_desc, &d->pts, &d->rb_int, &d->rb_dbl, &d->flush, &d->trace_fac, &d->trace_bs, &d->ptrace, &d->marg };
     for (int i = 0; i < 2; i++)
         if (d->tev[i])
             cudaEventDestroy(d->tev[i]);
@@ -871,6 +884,74 @@ ASAM_EXPORT int asam_linearize(asam_dev_t *d, int f_first, int f_count, const do
     if (flush_uploads(d))
         return 1;
     return run_linearize(d, a);
+}
+
+ASAM_EXPORT int asam_hessian_rebuild(asam_dev_t *d, int n_pose, const int32_t *pose, const int32_t *pose_ptr, int n_slot,
+                                     const int32_t *slot, const int32_t *slot_ptr, int n_ent, const int32_t *ent_f,
+                                     const double *ent_pts, const double *lam)
+{
+    if (n_pose < 0 || n_slot < 0 || n_ent < 0)
+        return set_err("asam_hessian_rebuild: %d poses, %d slots, %d entries", n_pose, n_slot, n_ent);
+    if (n_pose == 0 && n_slot == 0)
+        return 0;
+    CK(cudaSetDevice(d->device));
+    // ints: pose | pose_ptr | slot | slot_ptr | ent_f;  doubles: ent_pts | lam
+    const size_t ni = (size_t) n_pose + (n_pose + 1) + n_slot + (n_slot + 1) + n_ent;
+    const size_t nd = 6 * (size_t) n_ent + n_pose;
+    if (buf_reserve(d, d->rb_int, ni * sizeof(int), false, false) ||
+        buf_reserve(d, d->rb_dbl, (nd ? nd : 1) * sizeof(double), false, false))
+        return 1;
+    int *ip = (int *) d->rb_int.p;
+    double *dp = (double *) d->rb_dbl.p;
+    RebuildArgs a;
+    a.f_type = (const int *) d->f_type.p;
+    a.f_a = (const int *) d->f_a.p;
+    a.f_b = (const int *) d->f_b.p;
+    a.f_z = (const double *) d->f_z.p;
+    a.f_W = (const double *) d->f_W.p;
+    a.f_loss = (const double2 *) d->f_loss.p;
+    a.node2q = (const int *) d->node2q.p;
+    a.pose = ip;
+    a.pose_ptr = ip + n_pose;
+    a.slot = ip + 2 * (size_t) n_pose + 1;
+    a.slot_ptr = a.slot + n_slot;
+    a.ent_f = a.slot_ptr + n_slot + 1;
+    a.ent_pts = dp;
+    a.lam = dp + 6 * (size_t) n_ent;
+    a.Adiag = (double *) d->Adiag.p;
+    a.Aoff = (double *) d->Aoff.p;
+    a.Bq = (double *) d->Bq.p;
+    a.n_pose = n_pose;
+    a.n_slot = n_slot;
+    int rc = 0;
+    if (n_pose > 0) {
+        rc |= upload(d, (void *) a.pose, pose, (size_t) n_pose * sizeof(int));
+        rc |= upload(d, (void *) a.pose_ptr, pose_ptr, (size_t) (n_pose + 1) * sizeof(int));
+        rc |= upload(d, (void *) a.lam, lam, (size_t) n_pose * sizeof(double));
+    }
+    if (n_slot > 0) {
+        rc |= upload(d, (void *) a.slot, slot, (size_t) n_slot * sizeof(int));
+        rc |= upload(d, (void *) a.slot_ptr, slot_ptr, (size_t) (n_slot + 1) * sizeof(int));
+    }
+    if (n_ent > 0) {
+        rc |= upload(d, (void *) a.ent_f, ent_f, (size_t) n_ent * sizeof(int));
+        rc |= upload(d, (void *) a.ent_pts, ent_pts, 6 * (size_t) n_ent * sizeof(double));
+    }
+    if (rc)
+        return 1;
+    if (d->defer) {
+        if (d->npend >= ASAM_MAX_PENDING)
+            return set_err("too many deferred launches");
+        Pending &p = d->pend[d->npend++];
+        p.kind = 3;
+        p.grid = 0;
+        p.nleaf = 0;
+        p.rb = a;
+        return 0;
+    }
+    if (flush_uploads(d))
+        return 1;
+    return run_rebuild(d, a);
 }
 
 static int launch_factor(asam_dev *d, int ntasks, const int *tasks_dev, const int *nwait_dev, int with_leaves = 0,

@@ -380,6 +380,135 @@ __global__ void k_hessian_reset(double *Adiag, double *Aoff, double *Bq, int n_n
 }
 
 // ------------------------------------------------------------------------------------------
+// factor removal: the touched Hessian entries recomputed from the factors that remain
+// ------------------------------------------------------------------------------------------
+struct RebuildArgs {
+    const int *f_type, *f_a, *f_b;
+    const double *f_z, *f_W;
+    const double2 *f_loss;  // read by robust factors (type 32) only
+    const int *node2q;
+    const int *pose, *pose_ptr; // dirty pose i: incidence entries [pose_ptr[i], pose_ptr[i+1])
+    const int *slot, *slot_ptr; // dirty slot i: entries [slot_ptr[i], slot_ptr[i+1])
+    const int *ent_f;           // factor of each entry
+    const double *ent_pts;      // 6 doubles per entry: evaluation points of pose a, then b (priors: a only)
+    const double *lam;          // per dirty pose: the Tikhonov term on its diagonal
+    double *Adiag, *Aoff, *Bq;
+    int n_pose, n_slot;
+};
+
+// One factor at its evaluation points, with the maths of linearize_body: ca9 / cb9 = the upper triangle (r <= c) of
+// J_a'WJ_a / J_b'WJ_b packed in 6 + J'Wr (3), H = the off-diagonal block, "early" pose first, stored
+// [lower node id][higher node id].  A prior fills ca9 only.
+__device__ __forceinline__ void rebuild_factor(const RebuildArgs &a, const int f, const double *pts, double *ca9,
+                                               double *cb9, double *H)
+{
+    const int type = a.f_type[f];
+    double z[3], W[9];
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+        z[i] = a.f_z[3 * (size_t) f + i];
+#pragma unroll
+    for (int i = 0; i < 9; i++)
+        W[i] = a.f_W[9 * (size_t) f + i];
+    if (type == 2) {
+        const double r[3] = { z[0] - pts[0], z[1] - pts[1], d_mod2pi(z[2] - pts[2]) };
+        ca9[0] = W[0]; ca9[1] = W[1]; ca9[2] = W[2]; ca9[3] = W[4]; ca9[4] = W[5]; ca9[5] = W[8];
+        d_av(W, r, ca9 + 6);
+        return;
+    }
+    const int na = a.f_a[f], nb = a.f_b[f];
+    double Ja[9], Jb[9], r[3], JatW[9], JbtW[9], D[9];
+    d_xyt_eval(pts, pts + 3, z, Ja, Jb, r);
+    if (type == 32) {
+        const double2 lk = a.f_loss[f];
+        double X[3];
+        d_av(W, r, X);
+        const double w = d_loss_weight((int) lk.x, lk.y, r[0] * X[0] + r[1] * X[1] + r[2] * X[2]);
+#pragma unroll
+        for (int i = 0; i < 9; i++)
+            W[i] *= w;
+    }
+    d_atb(Ja, W, JatW);
+    d_atb(Jb, W, JbtW);
+    d_ab(JatW, Ja, D);
+    ca9[0] = D[0]; ca9[1] = D[1]; ca9[2] = D[2]; ca9[3] = D[4]; ca9[4] = D[5]; ca9[5] = D[8];
+    d_av(JatW, r, ca9 + 6);
+    d_ab(JbtW, Jb, D);
+    cb9[0] = D[0]; cb9[1] = D[1]; cb9[2] = D[2]; cb9[3] = D[4]; cb9[4] = D[5]; cb9[5] = D[8];
+    d_av(JbtW, r, cb9 + 6);
+    const int qa = a.node2q[na], qb = a.node2q[nb];
+    if (qa < qb)
+        d_ab(JatW, Jb, H);
+    else
+        d_ab(JbtW, Ja, H);
+    const int early = qa < qb ? na : nb;
+    if (early != (na < nb ? na : nb)) {
+        double tsw;
+        tsw = H[1]; H[1] = H[3]; H[3] = tsw;
+        tsw = H[2]; H[2] = H[6]; H[6] = tsw;
+        tsw = H[5]; H[5] = H[7]; H[7] = tsw;
+    }
+}
+
+// One warp per dirty pose: its lanes take the pose's entries in turn, each lane sums its share in list order, a fixed
+// butterfly adds the 32 partial sums, and lane 0 OVERWRITES Adiag (lambda + the sum on r <= c, 0 below) and Bq.  Then one
+// thread per dirty slot overwrites Aoff with its entries' blocks summed in list order (+0.0 for none).  No atomics: the
+// same lists give the same bits on every call; entries outside the lists are not touched.
+__global__ void __launch_bounds__(128) k_hessian_rebuild(RebuildArgs a)
+{
+    const int gt = blockIdx.x * blockDim.x + threadIdx.x;
+    const int w = gt >> 5, lane = gt & 31;
+    double ca9[9], cb9[9], H[9];
+    if (w < a.n_pose) {
+        const int p = a.pose[w];
+        double acc[9];
+#pragma unroll
+        for (int i = 0; i < 9; i++)
+            acc[i] = 0.0;
+        for (int e = a.pose_ptr[w] + lane; e < a.pose_ptr[w + 1]; e += 32) {
+            const int f = a.ent_f[e];
+            rebuild_factor(a, f, a.ent_pts + 6 * (size_t) e, ca9, cb9, H);
+            const bool is_b = a.f_type[f] != 2 && a.f_a[f] != p;
+#pragma unroll
+            for (int i = 0; i < 9; i++)
+                acc[i] += is_b ? cb9[i] : ca9[i];
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+            for (int i = 0; i < 9; i++)
+                acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
+        if (lane == 0) {
+            const double l = a.lam[w];
+            double *Ad = a.Adiag + 9 * (size_t) p;
+            Ad[0] = l + acc[0]; Ad[1] = acc[1]; Ad[2] = acc[2];
+            Ad[3] = 0.0; Ad[4] = l + acc[3]; Ad[5] = acc[4];
+            Ad[6] = 0.0; Ad[7] = 0.0; Ad[8] = l + acc[5];
+            double *Bn = a.Bq + 3 * (size_t) p;
+            Bn[0] = acc[6]; Bn[1] = acc[7]; Bn[2] = acc[8];
+        }
+        return;
+    }
+    const int si = (w - a.n_pose) * 32 + lane;
+    if (si >= a.n_slot)
+        return;
+    double S[9];
+#pragma unroll
+    for (int i = 0; i < 9; i++)
+        S[i] = 0.0;
+    for (int e = a.slot_ptr[si]; e < a.slot_ptr[si + 1]; e++) {
+        rebuild_factor(a, a.ent_f[e], a.ent_pts + 6 * (size_t) e, ca9, cb9, H);
+#pragma unroll
+        for (int i = 0; i < 9; i++)
+            S[i] += H[i];
+    }
+    double *Ao = a.Aoff + 9 * (size_t) a.slot[si];
+#pragma unroll
+    for (int i = 0; i < 9; i++)
+        Ao[i] = S[i];
+}
+
+// ------------------------------------------------------------------------------------------
 // kernel 2: persistent multifrontal factorisation (+ fused forward solve)
 // ------------------------------------------------------------------------------------------
 struct FacArgs {

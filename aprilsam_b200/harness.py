@@ -74,10 +74,16 @@ def _load(impl: str) -> C.CDLL:
     # covariance queries: only libraries that export them (never the reference build)
     for name, args in (("h_marginal_cov", [C.c_void_p, C.c_int, _ip, _dp]),
                        ("h_relative_cov", [C.c_void_p, C.c_int, C.c_int, _dp]),
-                       ("h_candidate_mahalanobis", [C.c_void_p, C.c_int, _ip, _ip, _dp, _dp, _dp, _dp])):
+                       ("h_candidate_mahalanobis", [C.c_void_p, C.c_int, _ip, _ip, _dp, _dp, _dp, _dp]),
+                       ("h_remove_factors", [C.c_void_p, C.c_int, _ip, C.c_int])):
         if hasattr(lib, name):
             getattr(lib, name).argtypes = args
             getattr(lib, name).restype = C.c_int
+    for name, args, res in (("h_param_create", [C.c_void_p], C.c_void_p), ("h_param_destroy", [C.c_void_p], None),
+                            ("h_swap_param", [C.c_void_p, C.c_void_p], C.c_void_p)):
+        if hasattr(lib, name):
+            getattr(lib, name).argtypes = args
+            getattr(lib, name).restype = res
     if hasattr(lib, "aprilsam_b200_last_error"):
         lib.aprilsam_b200_last_error.restype = C.c_char_p
     lib.h_relinearize.argtypes = [C.c_void_p, C.c_int]
@@ -266,6 +272,28 @@ class Harness:
                                             _d(cov) if with_cov else None) != 0:
             raise RuntimeError(self.lib.aprilsam_b200_last_error().decode())
         return (d2, cov) if with_cov else d2
+
+    def remove_factors(self, idx, keep: bool = False) -> None:
+        """aprilsam_b200_remove_factors: take factors idx out of the graph (the others keep their order) and update the
+        solution like an incremental step.  keep: the removed factors are handed back (and destroyed by the harness)
+        instead of being destroyed by the library.  Raises RuntimeError with the library's message when it returns -1."""
+        idx = np.ascontiguousarray(idx, dtype=np.int32).reshape(-1)
+        if self.lib.h_remove_factors(self.h, len(idx), _i(idx), int(keep)) != 0:
+            raise RuntimeError(self.lib.aprilsam_b200_last_error().decode())
+
+    def new_param(self) -> int:
+        """A further april_graph_cholesky_param_t for this graph (same settings); swap it in with swap_param."""
+        return self.lib.h_param_create(self.h)
+
+    def swap_param(self, p: int) -> int:
+        """Make p the param every call goes through; returns the one it replaces (free it with free_param)."""
+        return self.lib.h_swap_param(self.h, C.c_void_p(p))
+
+    def free_param(self, p: int) -> None:
+        self.lib.h_param_destroy(C.c_void_p(p))
+
+    def last_error(self) -> str:
+        return self.lib.aprilsam_b200_last_error().decode()
 
     def relinearize(self, i: int):
         self.lib.h_relinearize(self.h, i)

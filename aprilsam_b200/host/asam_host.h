@@ -161,6 +161,20 @@ int plan_build_with_order(plan_t *pl, asam_dev_t *dev, int N, int n_factors, con
 int plan_append(plan_t *pl, asam_dev_t *dev, int N, int n_factors, const int *ftype, const int *fa, const int *fb,
                 const int *marked_old, int n_marked, int **tasks_out, int **nwait_out, int **keep_out, int *ntasks_out);
 
+/* Re-factorisation list of a step that changes no structure (aprilsam_b200_remove_factors): marked = graph-node ids on
+ * the root paths (any order, all < pl->N).  tasks / nwait / keep (malloc'd, *ntasks_out entries) as plan_append gives
+ * them: the supernodes holding a marked pose, children first, nwait counting their marked children, keep =
+ * (poses before the first marked one << 16) | block rows, teams expanded (keep 0).  Emits no segments and uploads
+ * nothing; the plan is left as it was.  Returns 0. */
+int plan_refactor(plan_t *pl, const int *marked, int n_marked, int **tasks_out, int **nwait_out, int **keep_out,
+                  int *ntasks_out);
+
+/* Factors sorted_idx[0..n) (ascending, distinct, in [0, n_factors)) leave the plan: fslot and n_factors are compacted,
+ * the order of the other factors kept, and fslot is uploaded from sorted_idx[0] on (dev may be NULL).  Hessian slots
+ * stay; one that no remaining factor maps to is a dead zero block.  struct_hash becomes 0.  Nothing changes on an
+ * invalid list: 1 and the error text. */
+int plan_remove_factors(plan_t *pl, asam_dev_t *dev, int n, const int *sorted_idx);
+
 /* Modelled cost (columns x rows^2 + a latency term per front, the measure build_schedule balances
  * shards with) of re-factoring the distinct supernodes in tasks[0..ntasks) and of factoring every
  * supernode of the plan; feeds the escalation policy hook (aprilsam.h). */

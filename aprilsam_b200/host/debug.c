@@ -105,6 +105,28 @@ ASAM_API int asam_dbg_plan_append(void *p, int N, int F, const int *ftype, const
     return nt;
 }
 
+/* plan_refactor on a plan: returns ntasks (<= cap entries copied) */
+ASAM_API int asam_dbg_plan_refactor(void *p, const int *marked, int n_marked, int *tasks_out, int *nwait_out,
+                                    int *keep_out, int cap)
+{
+    int *tasks = NULL, *nwait = NULL, *keep = NULL, nt = 0;
+    plan_refactor((plan_t *) p, marked, n_marked, &tasks, &nwait, &keep, &nt);
+    int k = nt < cap ? nt : cap;
+    memcpy(tasks_out, tasks, sizeof(int) * (size_t) k);
+    memcpy(nwait_out, nwait, sizeof(int) * (size_t) k);
+    memcpy(keep_out, keep, sizeof(int) * (size_t) k);
+    free(tasks);
+    free(nwait);
+    free(keep);
+    return nt;
+}
+
+/* plan_remove_factors on a plan (no device): 0, or -1 with the error text */
+ASAM_API int asam_dbg_plan_remove_factors(void *p, int n, const int *sorted_idx)
+{
+    return plan_remove_factors((plan_t *) p, NULL, n, sorted_idx) ? -1 : 0;
+}
+
 /* info: N, nsn, n_slots, ipool_n, arena_n, max_m, nnz_l_blocks, n_levels, n_factors, n_bs_leaf */
 ASAM_API void asam_dbg_plan_info(void *p, int64_t *info, double *flops)
 {

@@ -1914,6 +1914,60 @@ int plan_append(plan_t *pl, asam_dev_t *dev, int N, int n_factors, const int *ft
     return rc;
 }
 
+/* ---- steps without structural change (factor removal) ---------------------------------------- */
+int plan_refactor(plan_t *pl, const int *marked, int n_marked, int **tasks_out, int **nwait_out, int **keep_out,
+                  int *ntasks_out)
+{
+    step_t st = { .N0 = pl->N, .F0 = pl->n_factors, .nsn0 = pl->nsn };
+    mark_supernodes(pl, &st, marked, n_marked);
+    st.nt = st.nm;
+    st.tasks = malloc(sizeof(int) * (size_t) (st.nt + 1));
+    st.nwait = malloc(sizeof(int) * (size_t) (st.nt + 1));
+    memcpy(st.tasks, st.msn, sizeof(int) * (size_t) st.nm);
+    for (int t = 0; t < st.nt; t++) {
+        int s = st.tasks[t], w = 0;
+        for (int c = 0; c < pl->snh[s].children.n; c++)
+            if (pl->mark_idx[pl->snh[s].children.p[c]] >= 0)
+                w++;
+        st.nwait[t] = pack_nwait(w, 0, 0);
+    }
+    expand_teams(pl, &st);
+    *tasks_out = st.tasks;
+    *nwait_out = st.nwait;
+    *keep_out = st.keep;
+    *ntasks_out = st.nt;
+    st.tasks = st.nwait = st.keep = NULL;
+    step_free(pl, &st);
+    return 0;
+}
+
+int plan_remove_factors(plan_t *pl, asam_dev_t *dev, int n, const int *sorted_idx)
+{
+    if (n < 1) {
+        asam_set_error("plan_remove_factors: n = %d", n);
+        return 1;
+    }
+    for (int k = 0; k < n; k++)
+        if (sorted_idx[k] < 0 || sorted_idx[k] >= pl->n_factors || (k > 0 && sorted_idx[k] <= sorted_idx[k - 1])) {
+            asam_set_error("plan_remove_factors: index %d (entry %d) is not ascending in [0, %d)", sorted_idx[k], k,
+                           pl->n_factors);
+            return 1;
+        }
+    const int F = pl->n_factors, first = sorted_idx[0];
+    for (int f = first, k = 0, out = first; f < F; f++) {
+        if (k < n && sorted_idx[k] == f) {
+            k++;
+            continue;
+        }
+        pl->fslot[out++] = pl->fslot[f];
+    }
+    pl->n_factors = F - n;
+    pl->struct_hash = 0; /* counts may match the next structure again (remove one, add one): never reuse */
+    if (dev && pl->n_factors > first && asam_upload_fslot(dev, first, pl->n_factors - first, pl->fslot + first))
+        return 1;
+    return 0;
+}
+
 int plan_marginal_paths(const plan_t *pl, int n, const int *nodes, asam_marg_path_t *out, int64_t *z_total,
                         int *hop_total)
 {

@@ -128,6 +128,11 @@ typedef struct gctx {
     double *zw; /* host mirror of what HBM holds: 12 doubles per factor (z[3], W[9]) */
     int32_t *floss; /* loss code and k per factor (0 / 0 without a robust loss); in HBM for robust factors */
     double *fk;
+    /* per factor: re-uploaded by gctx_verify_factors (an edit of z / W / loss) since the last batch linearised it, so
+     * HBM no longer holds what the Hessian was built from; all_stale: the mirror was rebuilt after a replaced factor */
+    unsigned char *fstale;
+    int n_stale, all_stale;
+    unsigned remove_epoch; /* aprilsam_b200_remove_factors calls on this graph (solvers that missed one are stale) */
     int fcap;
     double *stage; /* host staging for poses */
     int stage_cap;
@@ -177,6 +182,7 @@ static void gctx_unref(gctx_t *c)
     free(c->zw);
     free(c->floss);
     free(c->fk);
+    free(c->fstale);
     asam_dev_destroy(c->dev);
     free(c->ftype);
     free(c->fa);
@@ -219,7 +225,8 @@ static inline april_graph_factor_t *factor_at(april_graph_t *g, int i)
     return ((april_graph_factor_t **) g->factors->data)[i];
 }
 
-/* Mirror factors [c->nf_dev, F) into HBM (append-only API: aprilsam.h has no removal). */
+/* Mirror factors [c->nf_dev, F) into HBM (factors leave only through aprilsam_b200_remove_factors, which compacts the
+ * mirror itself). */
 static void gctx_sync_factors(gctx_t *c, april_graph_t *g)
 {
     int F = zarray_size(g->factors), N = zarray_size(g->nodes);
@@ -235,7 +242,9 @@ static void gctx_sync_factors(gctx_t *c, april_graph_t *g)
         c->zw = realloc(c->zw, sizeof(double) * 12 * (size_t) c->fcap);
         c->floss = realloc(c->floss, sizeof(int32_t) * (size_t) c->fcap);
         c->fk = realloc(c->fk, sizeof(double) * (size_t) c->fcap);
+        c->fstale = realloc(c->fstale, (size_t) c->fcap);
     }
+    memset(c->fstale + c->nf_dev, 0, (size_t) (F - c->nf_dev));
     int first = c->nf_dev, cnt = F - first;
     double *zw = malloc(sizeof(double) * 12 * (size_t) cnt);
     double *z = zw, *W = zw + 3 * (size_t) cnt;
@@ -311,6 +320,7 @@ static int gctx_verify_factors(gctx_t *c, april_graph_t *g, int upto)
             memcpy(m + 3, Wm->data, 9 * sizeof(double));
             c->floss[i] = loss;
             c->fk[i] = k;
+            c->fstale[i] = 1;
             changed = 1;
             if (i < lo)
                 lo = i;
@@ -318,10 +328,13 @@ static int gctx_verify_factors(gctx_t *c, april_graph_t *g, int upto)
                 hi = i;
         }
     }
-    if (structural)
+    if (structural) {
+        c->all_stale = 1;
         return 2;
+    }
     if (!changed)
         return 0;
+    c->n_stale = 1;
     /* re-upload the dirty range [lo, hi] (edits are usually a contiguous run or everything) */
     int cnt = hi - lo + 1;
     double *zw = malloc(sizeof(double) * 12 * (size_t) cnt);
@@ -360,7 +373,7 @@ ASAM_API double april_graph_chi2(april_graph_t *g)
 }
 
 /* ---- what the last incremental call asked of the kernels (tests; asam_dbg_record_steps) ------------- */
-enum { STEP_NONE = 0, STEP_SMALL = 1, STEP_PRUNED = 2, STEP_FULL = 3, STEP_FALLBACK = 4 };
+enum { STEP_NONE = 0, STEP_SMALL = 1, STEP_PRUNED = 2, STEP_FULL = 3, STEP_FALLBACK = 4, STEP_REMOVE = 5, STEP_REMOVE_FULL = 6 };
 
 typedef struct step_rec {
     int kind, escalated, ntasks, nbt;
@@ -419,6 +432,16 @@ typedef struct solver {
     aprilsam_b200_escalation_fn policy; /* deterministic escalation hook (aprilsam.h) */
     void *policy_user;
     step_rec_t rec; /* filled only while asam_dbg_record_steps is on */
+    /* what the Hessian in HBM was built from, for aprilsam_b200_remove_factors: the last batch put lam on the diagonal
+     * of poses [0, lam_n); priors added by incremental steps were evaluated at the states staged then (pr_st, 3
+     * doubles per entry, ascending factor index pr_f); a removal since the batch (removed) has left dead slots */
+    double lam;
+    int lam_n;
+    int *pr_f;
+    double *pr_st;
+    int n_pr, pr_cap;
+    int removed;
+    unsigned epoch; /* gc->remove_epoch as of this solver's last call */
 } solver_t;
 
 /* policies set before the first batch solve wait here for their solver (param -> fn) */
@@ -455,6 +478,8 @@ static void solver_destroy(solver_t *s)
     free(s->rec.keep);
     free(s->rec.bt);
     free(s->rec.bfirst);
+    free(s->pr_f);
+    free(s->pr_st);
     s->magic = 0;
     free(s);
 }
@@ -472,6 +497,7 @@ static solver_t *solver_get(april_graph_t *g, april_graph_cholesky_param_t *para
         s->magic = SOLVER_MAGIC;
         s->hdr.is_spd = 1;
         s->gc = gctx_get(g);
+        s->epoch = s->gc->remove_epoch;
         pthread_mutex_lock(&g_ctx_lock);
         s->gc->refs++;
         for (pending_policy_t **pp = &g_pending_policy; *pp; pp = &(*pp)->next)
@@ -704,6 +730,11 @@ ASAM_API void april_graph_cholesky(april_graph_t *graph, april_graph_cholesky_pa
         asam_set_timing(dev, 1);
         stamp(&tp, "begin");
     }
+    if (s->epoch != c->remove_epoch) { /* another solver removed factors: this plan may match the counts, not the graph */
+        s->plan_valid = 0;
+        s->tree_fresh = 0;
+        s->epoch = c->remove_epoch;
+    }
     int restarted = 0;
 restart:;
     const int F_mirrored = c->nf_dev < F ? c->nf_dev : F; /* already in HBM: checked while the kernels run */
@@ -820,6 +851,15 @@ restart:;
     memcpy(param->ordering, pl->order, sizeof(int) * (size_t) N);
     param->nreordering = N;
     param->factor_num = F;
+    /* this linearisation is what a later removal rebuilds from */
+    s->lam = param->tikhanov > 0 ? param->tikhanov : 0.0;
+    s->lam_n = N;
+    s->n_pr = 0;
+    s->removed = 0;
+    if (c->n_stale || c->all_stale) {
+        memset(c->fstale, 0, (size_t) c->nf_dev);
+        c->n_stale = c->all_stale = 0;
+    }
 
     double *x = solver_x(s, N);
     int fstatus = 0;
@@ -939,6 +979,179 @@ static void apply_solution(solver_t *s, search_tree_t *tr, const double *x, int 
 static void inc_general_fallback(april_graph_t *graph, april_graph_cholesky_param_t *param, solver_t *s, int N, int F,
                                  int F0);
 
+/* The solve of an incremental step or a removal (:563, :578-597), after its re-factorisation was recorded
+ * (asam_step_begin ... asam_factor): naffected > 5 back-substitutes every pose, otherwise only the supernodes the
+ * traversal visits (the marked poses and their children, closed under ancestors), each from its first wanted pose
+ * (bfirst).  Runs the recorded step, downloads x with the factorisation status and applies the solution
+ * (apply_solution).  A removal (removal = 1) never takes the one-launch k_step, which knows only the kernels of a step,
+ * and leaves the step counters of the host profile alone.  stage_off: doubles of the staging area still in use. */
+static void step_solve(april_graph_cholesky_param_t *param, solver_t *s, const int *marked, int n_marked, int ntasks,
+                       const int *nwait, int removal, int stage_off, stamps_t *tp)
+{
+    PROF_BEGIN();
+    gctx_t *c = s->gc;
+    asam_dev_t *dev = c->dev;
+    const plan_t *pl = &s->plan;
+    search_tree_t *tr = param->tr;
+    const int N = pl->N;
+    const char *where = removal ? "aprilsam_b200_remove_factors" : "april_graph_cholesky_inc";
+    double *x = solver_x(s, N);
+    int qbase = 0;
+    int fstatus = 0;
+    if (tr->naffected > 5) {
+        if (g_record_steps)
+            s->rec.kind = removal ? STEP_REMOVE_FULL : STEP_FULL;
+        DEV_OK(asam_backsolve_full(dev));
+        DEV_OK(asam_step_run(dev));
+        DEV_OK(asam_download_x_status(dev, 0, N, x, &fstatus));
+    } else {
+        /* visited = marked nodes + their children; close under ancestors.  Per supernode the first
+         * wanted pose: the back-substitution of a supernode stops there (cta_backsolve, jcol) */
+        if (pl->sn_cap > s->stamp_cap) {
+            s->sn_stamp = realloc(s->sn_stamp, sizeof(int) * (size_t) pl->sn_cap);
+            s->sn_jf = realloc(s->sn_jf, sizeof(int) * (size_t) pl->sn_cap);
+            s->sn_bt = realloc(s->sn_bt, sizeof(int) * 2 * (size_t) pl->sn_cap);
+            memset(s->sn_stamp + s->stamp_cap, 0, sizeof(int) * (size_t) (pl->sn_cap - s->stamp_cap));
+            s->stamp_cap = pl->sn_cap;
+        }
+        if (++s->stamp_epoch == INT_MAX) {
+            memset(s->sn_stamp, 0, sizeof(int) * (size_t) s->stamp_cap);
+            s->stamp_epoch = 1;
+        }
+        int *stamp = s->sn_stamp, *jf = s->sn_jf, *bt = s->sn_bt;
+        const int ep = s->stamp_epoch;
+        int nbt = 0, qmin = N;
+        for (int i = 0; i < n_marked; i++) {
+            search_tree_node_t *node = &tr->nodes[marked[i]];
+            for (int ci = -1; ci < node->nchildren; ci++) {
+                int v = ci < 0 ? marked[i] : node->children[ci];
+                int q = pl->node2q[v], sn0 = pl->sn_of_q[q], sn = sn0;
+                while (sn >= 0 && stamp[sn] != ep) {
+                    stamp[sn] = ep;
+                    jf[sn] = pl->desc[sn].cb;
+                    bt[nbt++] = sn;
+                    if (pl->desc[sn].first < qmin)
+                        qmin = pl->desc[sn].first;
+                    sn = pl->desc[sn].parent;
+                }
+                if (q - pl->desc[sn0].first < jf[sn0])
+                    jf[sn0] = q - pl->desc[sn0].first;
+            }
+        }
+        /* parents before children: descending supernode id */
+        for (int i = 1; i < nbt; i++) {
+            int v = bt[i], j = i - 1;
+            while (j >= 0 && bt[j] < v) {
+                bt[j + 1] = bt[j];
+                j--;
+            }
+            bt[j + 1] = v;
+        }
+        int *bfirst = bt + pl->sn_cap;
+        for (int i = 0; i < nbt; i++)
+            bfirst[i] = jf[bt[i]] < pl->desc[bt[i]].cb ? jf[bt[i]] : 0;
+        DEV_OK(asam_backsolve(dev, nbt, bt, bfirst));
+        /* a handful of single-CTA fronts: the whole step in ONE launch, results through pinned memory */
+        int small = !removal && nbt <= ASAM_SMALL_MAX_BS && ntasks <= ASAM_SMALL_MAX_TASKS && asam_step_small_supported(dev);
+        for (int t = 0; small && t < ntasks; t++)
+            small = ((nwait[t] >> 24) & 0x7f) <= 1;
+        if (small) {
+            int xd = 0;
+            for (int i = 0; i < nbt; i++)
+                xd += 3 * pl->desc[bt[i]].cb;
+            double *xc = gctx_stage(c, stage_off + xd) + stage_off; /* behind the evaluation points */
+            int rs = asam_step_run_small(dev, xc, xd, &fstatus);
+            if (rs == 0) {
+                for (int i = 0, off = 0; i < nbt; i++) {
+                    const asam_sn_desc_t *sd = &pl->desc[bt[i]];
+                    memcpy(x + 3 * (size_t) sd->first, xc + off, sizeof(double) * 3 * (size_t) sd->cb);
+                    off += 3 * sd->cb;
+                }
+                qbase = 0;
+                g_prof[18] += 1;
+                g_prof[19] += ntasks;
+                g_prof[20] += nbt;
+                g_prof[21] += xd;
+            } else if (rs == 2) {
+                small = 0;
+            } else {
+                asam_fatal("%s: %s", where, asam_last_error());
+            }
+        }
+        if (!small) {
+            DEV_OK(asam_step_run(dev));
+            qbase = qmin;
+            DEV_OK(asam_download_x_status(dev, qbase, N - qbase, x, &fstatus));
+        }
+        if (g_record_steps) {
+            s->rec.kind = removal ? STEP_REMOVE : small ? STEP_SMALL : STEP_PRUNED;
+            rec_bt(&s->rec, nbt, bt, bfirst);
+        }
+    }
+    if (!removal)
+        PROF_LAP(4);
+    report_factor_status(s, fstatus, where);
+    if (!removal)
+        PROF_LAP(5);
+    if (param->show_timing)
+        stamp(tp, "H2D, kernels, D2H of solution");
+    apply_solution(s, tr, x, qbase);
+    if (!removal) {
+        PROF_LAP(6);
+        if (tr->naffected > 5)
+            g_prof[17] += 1;
+    }
+    if (param->show_timing) {
+        stamp(tp, "solve_node bookkeeping");
+        stamps_display(tp, dev);
+    }
+}
+
+/* Priors added by incremental steps: the state each was evaluated at (a removal rebuilds them there) */
+static void prior_record(solver_t *s, int f, const double *st)
+{
+    if (s->n_pr == s->pr_cap) {
+        s->pr_cap = s->pr_cap ? 2 * s->pr_cap : 16;
+        s->pr_f = realloc(s->pr_f, sizeof(int) * (size_t) s->pr_cap);
+        s->pr_st = realloc(s->pr_st, sizeof(double) * 3 * (size_t) s->pr_cap);
+    }
+    s->pr_f[s->n_pr] = f;
+    memcpy(s->pr_st + 3 * (size_t) s->n_pr++, st, 3 * sizeof(double));
+}
+
+/* The recorded state of prior f, or NULL for a prior present at the last batch (evaluated at its l_point) */
+static const double *prior_point(const solver_t *s, int f)
+{
+    int lo = 0, hi = s->n_pr;
+    while (lo < hi) {
+        int mid = (lo + hi) / 2;
+        if (s->pr_f[mid] < f)
+            lo = mid + 1;
+        else
+            hi = mid;
+    }
+    return lo < s->n_pr && s->pr_f[lo] == f ? s->pr_st + 3 * (size_t) lo : NULL;
+}
+
+static void step_escalate(april_graph_t *graph, april_graph_cholesky_param_t *param);
+
+/* The points factor f of the mirror was evaluated at for the Hessian in HBM (a then b): the l_points of its poses for an
+ * xyt factor (plain or robust), the recorded state for a prior added by a step, the l_point of its pose for a prior
+ * present at the last batch */
+static void eval_point(const solver_t *s, april_graph_t *g, int f, double *pts6)
+{
+    const gctx_t *c = s->gc;
+    if (asam_two_pose_type(c->ftype[f])) {
+        memcpy(pts6, node_at(g, c->fa[f])->l_point, 3 * sizeof(double));
+        memcpy(pts6 + 3, node_at(g, c->fb[f])->l_point, 3 * sizeof(double));
+        return;
+    }
+    const double *st = prior_point(s, f);
+    memcpy(pts6, st ? st : node_at(g, c->fa[f])->l_point, 3 * sizeof(double));
+    memset(pts6 + 3, 0, 3 * sizeof(double));
+}
+
+
 ASAM_API void april_graph_cholesky_inc(april_graph_t *graph, april_graph_cholesky_param_t *param)
 {
     int N = zarray_size(graph->nodes), F = zarray_size(graph->factors);
@@ -946,9 +1159,14 @@ ASAM_API void april_graph_cholesky_inc(april_graph_t *graph, april_graph_cholesk
         return;
     if (!param->chol)
         return;
+    solver_t *s = solver_of(param);
+    if (s->gc->graph == graph && s->epoch != s->gc->remove_epoch) {
+        asam_set_error("april_graph_cholesky_inc: factors were removed from this graph through another param since this "
+                       "one last solved it; nothing was done (solve with april_graph_cholesky first)");
+        return;
+    }
     if (param->factor_num == F)
         return;
-    solver_t *s = solver_of(param);
     if (s->gc->graph != graph || !s->plan_valid || !param->tr)
         asam_fatal("april_graph_cholesky_inc: param does not continue a batch solve of this graph");
     gctx_t *c = s->gc;
@@ -1038,6 +1256,7 @@ ASAM_API void april_graph_cholesky_inc(april_graph_t *graph, april_graph_cholesk
         } else {
             memcpy(pts + 6 * (size_t) k, node_at(graph, c->fa[f])->state, 3 * sizeof(double));
             memset(pts + 6 * (size_t) k + 3, 0, 3 * sizeof(double));
+            prior_record(s, f, pts + 6 * (size_t) k);
         }
     }
 
@@ -1079,115 +1298,7 @@ ASAM_API void april_graph_cholesky_inc(april_graph_t *graph, april_graph_cholesk
     param->nreordering = N;
     PROF_LAP(3);
 
-    /* solve (:563, :578-597): which supernodes does the traversal need? */
-    {
-        double *x = solver_x(s, N);
-        int qbase = 0;
-        int fstatus = 0;
-        if (tr->naffected > 5) {
-            if (g_record_steps)
-                s->rec.kind = STEP_FULL;
-            DEV_OK(asam_backsolve_full(dev));
-            DEV_OK(asam_step_run(dev));
-            DEV_OK(asam_download_x_status(dev, 0, N, x, &fstatus));
-        } else {
-            /* visited = marked nodes + their children; close under ancestors.  Per supernode the first
-             * wanted pose: the back-substitution of a supernode stops there (cta_backsolve, jcol) */
-            if (pl->sn_cap > s->stamp_cap) {
-                s->sn_stamp = realloc(s->sn_stamp, sizeof(int) * (size_t) pl->sn_cap);
-                s->sn_jf = realloc(s->sn_jf, sizeof(int) * (size_t) pl->sn_cap);
-                s->sn_bt = realloc(s->sn_bt, sizeof(int) * 2 * (size_t) pl->sn_cap);
-                memset(s->sn_stamp + s->stamp_cap, 0, sizeof(int) * (size_t) (pl->sn_cap - s->stamp_cap));
-                s->stamp_cap = pl->sn_cap;
-            }
-            if (++s->stamp_epoch == INT_MAX) {
-                memset(s->sn_stamp, 0, sizeof(int) * (size_t) s->stamp_cap);
-                s->stamp_epoch = 1;
-            }
-            int *stamp = s->sn_stamp, *jf = s->sn_jf, *bt = s->sn_bt;
-            const int ep = s->stamp_epoch;
-            int nbt = 0, qmin = N;
-            for (int i = 0; i < n_marked; i++) {
-                search_tree_node_t *node = &tr->nodes[marked[i]];
-                for (int ci = -1; ci < node->nchildren; ci++) {
-                    int v = ci < 0 ? marked[i] : node->children[ci];
-                    int q = pl->node2q[v], sn0 = pl->sn_of_q[q], sn = sn0;
-                    while (sn >= 0 && stamp[sn] != ep) {
-                        stamp[sn] = ep;
-                        jf[sn] = pl->desc[sn].cb;
-                        bt[nbt++] = sn;
-                        if (pl->desc[sn].first < qmin)
-                            qmin = pl->desc[sn].first;
-                        sn = pl->desc[sn].parent;
-                    }
-                    if (q - pl->desc[sn0].first < jf[sn0])
-                        jf[sn0] = q - pl->desc[sn0].first;
-                }
-            }
-            /* parents before children: descending supernode id */
-            for (int i = 1; i < nbt; i++) {
-                int v = bt[i], j = i - 1;
-                while (j >= 0 && bt[j] < v) {
-                    bt[j + 1] = bt[j];
-                    j--;
-                }
-                bt[j + 1] = v;
-            }
-            int *bfirst = bt + pl->sn_cap;
-            for (int i = 0; i < nbt; i++)
-                bfirst[i] = jf[bt[i]] < pl->desc[bt[i]].cb ? jf[bt[i]] : 0;
-            DEV_OK(asam_backsolve(dev, nbt, bt, bfirst));
-            /* a handful of single-CTA fronts: the whole step in ONE launch, results through pinned memory */
-            int small = nbt <= ASAM_SMALL_MAX_BS && ntasks <= ASAM_SMALL_MAX_TASKS && asam_step_small_supported(dev);
-            for (int t = 0; small && t < ntasks; t++)
-                small = ((nwait[t] >> 24) & 0x7f) <= 1;
-            if (small) {
-                int xd = 0;
-                for (int i = 0; i < nbt; i++)
-                    xd += 3 * pl->desc[bt[i]].cb;
-                double *xc = gctx_stage(c, 6 * nf + xd) + 6 * (size_t) nf; /* behind the evaluation points */
-                int rs = asam_step_run_small(dev, xc, xd, &fstatus);
-                if (rs == 0) {
-                    for (int i = 0, off = 0; i < nbt; i++) {
-                        const asam_sn_desc_t *sd = &pl->desc[bt[i]];
-                        memcpy(x + 3 * (size_t) sd->first, xc + off, sizeof(double) * 3 * (size_t) sd->cb);
-                        off += 3 * sd->cb;
-                    }
-                    qbase = 0;
-                    g_prof[18] += 1;
-                    g_prof[19] += ntasks;
-                    g_prof[20] += nbt;
-                    g_prof[21] += xd;
-                } else if (rs == 2) {
-                    small = 0;
-                } else {
-                    asam_fatal("april_graph_cholesky_inc: %s", asam_last_error());
-                }
-            }
-            if (!small) {
-                DEV_OK(asam_step_run(dev));
-                qbase = qmin;
-                DEV_OK(asam_download_x_status(dev, qbase, N - qbase, x, &fstatus));
-            }
-            if (g_record_steps) {
-                s->rec.kind = small ? STEP_SMALL : STEP_PRUNED;
-                rec_bt(&s->rec, nbt, bt, bfirst);
-            }
-        }
-        PROF_LAP(4);
-        report_factor_status(s, fstatus, "april_graph_cholesky_inc");
-        PROF_LAP(5);
-        if (param->show_timing)
-            stamp(&tp, "H2D, kernels, D2H of solution");
-        apply_solution(s, tr, x, qbase);
-        PROF_LAP(6);
-        if (tr->naffected > 5)
-            g_prof[17] += 1;
-        if (param->show_timing) {
-            stamp(&tp, "solve_node bookkeeping");
-            stamps_display(&tp, dev);
-        }
-    }
+    step_solve(param, s, marked, n_marked, ntasks, nwait, 0, 6 * nf, &tp);
     free(tasks);
     free(nwait);
     free(keep);
@@ -1196,7 +1307,12 @@ ASAM_API void april_graph_cholesky_inc(april_graph_t *graph, april_graph_cholesk
         param->tr->start_over = INT_MAX;
 
 escalate:
-    /* too many poses moved since the last batch: relinearise everything (:566-575) */
+    step_escalate(graph, param);
+}
+
+/* too many poses moved since the last batch: relinearise everything (:566-575) */
+static void step_escalate(april_graph_t *graph, april_graph_cholesky_param_t *param)
+{
     if (param->tr->start_over > param->nthreshold) {
         free(param->ordering);
         param->ordering = NULL;
@@ -1231,9 +1347,21 @@ static void inc_general_fallback(april_graph_t *graph, april_graph_cholesky_para
     if (plan_build_with_order(pl, dev, N, F, c->ftype, c->fa, c->fb, param->ordering, N0) != 0)
         asam_fatal("april_graph_cholesky_inc: %s %s", g_error, asam_last_error());
     s->plan.struct_hash = 0; /* order differs from a fresh batch: never reuse for one */
-    DEV_OK(asam_hessian_clear_range(dev, N0, N - N0, old_slots, pl->n_slots - old_slots));
-    double *pts = c->stage; /* filled by the caller */
-    DEV_OK(asam_linearize(dev, F0, nf, pts));
+    if (s->removed) {
+        /* a removal left slots that the rebuild dropped, so later slots were renumbered: the whole Hessian is
+         * built again, every factor at the point it was evaluated at (no relinearisation) */
+        double *all = malloc(sizeof(double) * 6 * (size_t) F);
+        for (int f = 0; f < F; f++)
+            eval_point(s, graph, f, all + 6 * (size_t) f);
+        DEV_OK(asam_hessian_reset(dev, N, pl->n_slots, s->lam_n, s->lam));
+        DEV_OK(asam_linearize(dev, 0, F, all));
+        free(all);
+        s->removed = 0;
+    } else {
+        DEV_OK(asam_hessian_clear_range(dev, N0, N - N0, old_slots, pl->n_slots - old_slots));
+        double *pts = c->stage; /* filled by the caller */
+        DEV_OK(asam_linearize(dev, F0, nf, pts));
+    }
     DEV_OK(asam_factor_full(dev));
     DEV_OK(asam_backsolve_full(dev));
     double *x = solver_x(s, N);
@@ -1276,6 +1404,428 @@ ASAM_API void april_graph_cholesky_inc_solver(april_graph_t *graph, april_graph_
     param->tr->naffected = 6;
     apply_solution(s, param->tr, x, 0);
     param->tr->naffected = keep;
+}
+
+/* ---- factor removal (extension) ------------------------------------------------------------------------------ */
+static gctx_t *gctx_find(april_graph_t *g)
+{
+    pthread_mutex_lock(&g_ctx_lock);
+    gctx_t *hit = NULL;
+    for (gctx_t *c = g_ctx_list; c; c = c->next)
+        if (c->graph == g) {
+            hit = c;
+            break;
+        }
+    pthread_mutex_unlock(&g_ctx_lock);
+    return hit;
+}
+
+/* Drop the removed factors (sorted[0..n), ascending) from the host mirror and upload what moved: HBM then holds the
+ * remaining factors in their new order.  Values come from the mirror, not from the caller's structs, so an edit the
+ * mirror has not seen yet stays unseen until the next batch checks it.  Factors not mirrored yet are skipped. */
+static void gctx_remove_factors(gctx_t *c, int n, const int *sorted)
+{
+    int m = 0;
+    while (m < n && sorted[m] < c->nf_dev)
+        m++;
+    if (m == 0)
+        return;
+    const int first = sorted[0], F = c->nf_dev;
+    int out = first;
+    for (int f = first, k = 0; f < F; f++) {
+        if (k < m && sorted[k] == f) {
+            k++;
+            continue;
+        }
+        c->ftype[out] = c->ftype[f];
+        c->fa[out] = c->fa[f];
+        c->fb[out] = c->fb[f];
+        memcpy(c->zw + 12 * (size_t) out, c->zw + 12 * (size_t) f, 12 * sizeof(double));
+        c->floss[out] = c->floss[f];
+        c->fk[out] = c->fk[f];
+        c->fstale[out] = c->fstale[f];
+        out++;
+    }
+    c->nf_dev = out;
+    const int cnt = out - first;
+    if (cnt <= 0)
+        return;
+    double *zw = malloc(sizeof(double) * 12 * (size_t) cnt);
+    double *z = zw, *W = zw + 3 * (size_t) cnt;
+    int robust = 0;
+    for (int k = 0; k < cnt; k++) {
+        memcpy(z + 3 * (size_t) k, c->zw + 12 * (size_t) (first + k), 3 * sizeof(double));
+        memcpy(W + 9 * (size_t) k, c->zw + 12 * (size_t) (first + k) + 3, 9 * sizeof(double));
+        robust |= c->floss[first + k] != 0;
+    }
+    DEV_OK(asam_upload_factors(c->dev, first, cnt, c->ftype + first, c->fa + first, c->fb + first, z, W));
+    if (robust)
+        DEV_OK(asam_upload_loss(c->dev, first, cnt, c->floss + first, c->fk + first));
+    free(zw);
+}
+
+/* Take the factors out of graph->factors, the others keeping their order; hand them to the caller (factor_idx order)
+ * or destroy them */
+static void graph_splice(april_graph_t *g, int n, const int *factor_idx, const int *sorted,
+                         april_graph_factor_t **removed_out)
+{
+    april_graph_factor_t **fs = (april_graph_factor_t **) g->factors->data;
+    const int F = zarray_size(g->factors);
+    for (int k = 0; k < n; k++) {
+        if (removed_out)
+            removed_out[k] = fs[factor_idx[k]];
+        else
+            fs[factor_idx[k]]->destroy(fs[factor_idx[k]]);
+    }
+    int out = sorted[0];
+    for (int f = sorted[0], k = 0; f < F; f++) {
+        if (k < n && sorted[k] == f) {
+            k++;
+            continue;
+        }
+        fs[out++] = fs[f];
+    }
+    g->factors->size = out;
+}
+
+static int cmp_int_asc(const void *a, const void *b)
+{
+    int x = *(const int *) a, y = *(const int *) b;
+    return (x > y) - (x < y);
+}
+
+/* sorted lookup: index of v in p[0..n) or -1 */
+static int find_int(const int *p, int n, int v)
+{
+    int lo = 0, hi = n;
+    while (lo < hi) {
+        int mid = (lo + hi) / 2;
+        if (p[mid] < v)
+            lo = mid + 1;
+        else
+            hi = mid;
+    }
+    return lo < n && p[lo] == v ? lo : -1;
+}
+
+/* Is every pose of `dirty` still anchored once the removed factors (rm[f] = 1) are gone: a pose with a Tikhonov term
+ * (it existed at the last batch, lambda > 0) or a remaining prior, or one the remaining factors connect to such a pose?
+ * Breadth-first from each dirty pose, stopping at the first anchored pose.  Returns the first pose left without an
+ * anchor, or -1. */
+static int unanchored_pose(const solver_t *s, int N, int F, const unsigned char *rm, const int *dirty, int n_dirty,
+                           const unsigned char *dirty_prior)
+{
+    const gctx_t *c = s->gc;
+    const int lam_on = s->lam > 0.0;
+    int need = 0;
+    for (int i = 0; i < n_dirty && !need; i++)
+        need = !((lam_on && dirty[i] < s->lam_n) || dirty_prior[i]);
+    if (!need)
+        return -1;
+    /* adjacency of the remaining factors; a prior marks its pose */
+    int *deg = calloc((size_t) N + 1, sizeof(int));
+    unsigned char *prior = calloc((size_t) N, 1);
+    for (int f = 0; f < F; f++) {
+        if (rm[f])
+            continue;
+        if (asam_two_pose_type(c->ftype[f])) {
+            deg[c->fa[f] + 1]++;
+            deg[c->fb[f] + 1]++;
+        } else {
+            prior[c->fa[f]] = 1;
+        }
+    }
+    for (int i = 0; i < N; i++)
+        deg[i + 1] += deg[i];
+    int *adj = malloc(sizeof(int) * (size_t) (deg[N] + 1)), *fill = malloc(sizeof(int) * (size_t) N);
+    memcpy(fill, deg, sizeof(int) * (size_t) N);
+    for (int f = 0; f < F; f++)
+        if (!rm[f] && asam_two_pose_type(c->ftype[f])) {
+            adj[fill[c->fa[f]]++] = c->fb[f];
+            adj[fill[c->fb[f]]++] = c->fa[f];
+        }
+    int *seen = calloc((size_t) N, sizeof(int)), *queue = fill; /* fill is free again */
+    int bad = -1;
+    for (int i = 0; i < n_dirty && bad < 0; i++) {
+        int head = 0, tail = 0, found = 0;
+        queue[tail++] = dirty[i];
+        seen[dirty[i]] = i + 1;
+        while (head < tail && !found) {
+            int v = queue[head++];
+            if ((lam_on && v < s->lam_n) || prior[v]) {
+                found = 1;
+                break;
+            }
+            for (int e = deg[v]; e < deg[v + 1]; e++)
+                if (seen[adj[e]] != i + 1) {
+                    seen[adj[e]] = i + 1;
+                    queue[tail++] = adj[e];
+                }
+        }
+        if (!found)
+            bad = dirty[i];
+    }
+    free(deg);
+    free(prior);
+    free(adj);
+    free(fill);
+    free(seen);
+    return bad;
+}
+
+ASAM_API int aprilsam_b200_remove_factors(april_graph_t *graph, april_graph_cholesky_param_t *param, int n,
+                                          const int *factor_idx, april_graph_factor_t **removed_out)
+{
+    const char *fn = "aprilsam_b200_remove_factors";
+    if (!graph || !param || !factor_idx || n < 1) {
+        asam_set_error("%s: NULL graph / param / factor_idx or n < 1", fn);
+        return -1;
+    }
+    const int N = zarray_size(graph->nodes), F = zarray_size(graph->factors);
+    int *idx = malloc(sizeof(int) * (size_t) n);
+    for (int k = 0; k < n; k++) {
+        if (factor_idx[k] < 0 || factor_idx[k] >= F) {
+            asam_set_error("%s: factor index %d (entry %d) is not in [0, %d)", fn, factor_idx[k], k, F);
+            free(idx);
+            return -1;
+        }
+        idx[k] = factor_idx[k];
+    }
+    qsort(idx, (size_t) n, sizeof(int), cmp_int_asc);
+    for (int k = 1; k < n; k++)
+        if (idx[k] == idx[k - 1]) {
+            asam_set_error("%s: factor index %d is listed twice", fn, idx[k]);
+            free(idx);
+            return -1;
+        }
+    if (!param->chol) { /* never solved: only the splice (and the mirror of a graph another param solved) */
+        gctx_t *c = gctx_find(graph);
+        if (c) {
+            gctx_remove_factors(c, n, idx);
+            c->remove_epoch++;
+        }
+        graph_splice(graph, n, factor_idx, idx, removed_out);
+        free(idx);
+        return 0;
+    }
+    solver_t *s = solver_of(param);
+    gctx_t *c = s->gc;
+    const char *why = NULL;
+    if (c->graph != graph)
+        why = "param does not continue a solve of this graph";
+    else if (!s->plan_valid)
+        why = "the plan was dropped (aprilsam_b200_invalidate_plan); solve again first";
+    else if (s->epoch != c->remove_epoch)
+        why = "factors were removed from this graph through another param since this one last solved it; solve with "
+              "april_graph_cholesky first";
+    else if (s->plan.world > 1)
+        why = "the last batch solve was sharded over several GPUs; removal continues single-GPU solves only";
+    else if (!param->tr || N != s->plan.N || F != s->plan.n_factors || F != param->factor_num || F != c->nf_dev)
+        why = "poses or factors were added since the last solve (call april_graph_cholesky_inc first)";
+    else if (c->all_stale)
+        why = "a factor was replaced since the last batch solve (its HBM mirror no longer matches the linearised "
+              "Hessian); solve with april_graph_cholesky first";
+    if (why) {
+        asam_set_error("%s: %s", fn, why);
+        free(idx);
+        return -1;
+    }
+
+    /* ---- validation on the unchanged state: dirty poses and slots, the remaining factors on them ---- */
+    plan_t *pl = &s->plan;
+    double t_scan = prof_now();
+    int *dirty = malloc(sizeof(int) * 2 * (size_t) n), n_dirty = 0;
+    int *dslot = malloc(sizeof(int) * (size_t) n), n_dslot = 0;
+    for (int k = 0; k < n; k++) {
+        int f = idx[k];
+        dirty[n_dirty++] = c->fa[f];
+        if (asam_two_pose_type(c->ftype[f])) {
+            dirty[n_dirty++] = c->fb[f];
+            dslot[n_dslot++] = pl->fslot[f];
+        }
+    }
+    qsort(dirty, (size_t) n_dirty, sizeof(int), cmp_int_asc);
+    qsort(dslot, (size_t) n_dslot, sizeof(int), cmp_int_asc);
+    int w = 0;
+    for (int i = 0; i < n_dirty; i++)
+        if (i == 0 || dirty[i] != dirty[i - 1])
+            dirty[w++] = dirty[i];
+    n_dirty = w;
+    w = 0;
+    for (int i = 0; i < n_dslot; i++)
+        if (i == 0 || dslot[i] != dslot[i - 1])
+            dslot[w++] = dslot[i];
+    n_dslot = w;
+    /* one scan of the factor list: per dirty pose and per dirty slot, its remaining factors in index order
+     * (entries hold the index AFTER compaction) */
+    unsigned char *rm = calloc((size_t) F, 1);
+    for (int k = 0; k < n; k++)
+        rm[idx[k]] = 1;
+    int *pcnt = calloc((size_t) n_dirty + 1, sizeof(int)), *scnt = calloc((size_t) n_dslot + 1, sizeof(int));
+    unsigned char *dprior = calloc((size_t) n_dirty + 1, 1);
+    ivec_t hit = { 0 }; /* (f, pose index or -1, slot index or -1) triples */
+    int stale = -1;
+    for (int f = 0; f < F; f++) {
+        if (rm[f])
+            continue;
+        int two = asam_two_pose_type(c->ftype[f]);
+        int ia = find_int(dirty, n_dirty, c->fa[f]), ib = two ? find_int(dirty, n_dirty, c->fb[f]) : -1;
+        if (ia < 0 && ib < 0)
+            continue;
+        int is = two && ia >= 0 && ib >= 0 ? find_int(dslot, n_dslot, pl->fslot[f]) : -1;
+        if (c->fstale[f] && stale < 0)
+            stale = f;
+        ivec_push(&hit, f);
+        ivec_push(&hit, ia);
+        ivec_push(&hit, ib);
+        ivec_push(&hit, is);
+        if (ia >= 0)
+            pcnt[ia]++;
+        if (ib >= 0)
+            pcnt[ib]++;
+        if (is >= 0)
+            scnt[is]++;
+        if (!two)
+            dprior[ia] = 1;
+    }
+    int bad = stale < 0 ? unanchored_pose(s, N, F, rm, dirty, n_dirty, dprior) : -1;
+    t_scan = prof_now() - t_scan;
+    if (stale >= 0 || bad >= 0) {
+        if (stale >= 0)
+            asam_set_error("%s: factor %d, which shares a pose with a removed factor, was edited since the last batch "
+                           "solve (its HBM mirror no longer holds the values the Hessian was built from); solve with "
+                           "april_graph_cholesky first", fn, stale);
+        else
+            asam_set_error("%s: pose %d would be left unconstrained: it was created after the last batch solve and no "
+                           "remaining factor connects it to a pose of that batch or to a prior", fn, bad);
+        free(idx); free(dirty); free(dslot); free(rm); free(pcnt); free(scnt); free(dprior); ivec_free(&hit);
+        return -1;
+    }
+
+    /* ---- from here on the removal happens ---- */
+    g_prof[22] += t_scan;
+    g_prof[23] += 1;
+    asam_dev_t *dev = c->dev;
+    search_tree_t *tr = param->tr;
+    stamps_t tp = { .n = 0 };
+    if (param->show_timing) {
+        asam_set_timing(dev, 1);
+        stamp(&tp, "begin");
+    }
+    s->tree_fresh = 0;
+    if (g_record_steps) {
+        s->rec.kind = STEP_NONE;
+        s->rec.escalated = 0;
+        s->rec.ntasks = s->rec.nbt = 0;
+    }
+    /* root paths of the removed factors' poses, as if they had been added by a step (:482-498) */
+    int *marked = solver_scratch(s, 2 * N + 16) + N + 8; /* upper half: apply_solution uses the lower */
+    int n_marked = 0;
+    tr->naffected = 0;
+    for (int k = 0; k < n; k++) {
+        int f = idx[k], ends[2] = { c->fa[f], c->fb[f] };
+        for (int z0 = 0; z0 < (asam_two_pose_type(c->ftype[f]) ? 2 : 1); z0++) {
+            search_tree_node_t *node = &tr->nodes[ends[z0]];
+            while (!node->label_changed) {
+                node->label_changed = 1;
+                tr->naffected++;
+                marked[n_marked++] = (int) (node - tr->nodes);
+                if (node->parent != -1)
+                    node = &tr->nodes[node->parent];
+                else
+                    break;
+            }
+        }
+    }
+    /* the rebuild tables (evaluation points read before the mirror moves) */
+    const int n_hit = hit.n / 4;
+    int *pptr = malloc(sizeof(int) * ((size_t) n_dirty + 1)), *sptr = malloc(sizeof(int) * ((size_t) n_dslot + 1));
+    pptr[0] = 0;
+    for (int i = 0; i < n_dirty; i++)
+        pptr[i + 1] = pptr[i] + pcnt[i];
+    sptr[0] = pptr[n_dirty];
+    for (int i = 0; i < n_dslot; i++)
+        sptr[i + 1] = sptr[i] + scnt[i];
+    const int n_ent = sptr[n_dslot];
+    int *ent_f = malloc(sizeof(int) * ((size_t) n_ent + 1));
+    double *ent_pts = malloc(sizeof(double) * 6 * ((size_t) n_ent + 1));
+    double *lamv = malloc(sizeof(double) * ((size_t) n_dirty + 1));
+    memcpy(pcnt, pptr, sizeof(int) * (size_t) n_dirty); /* fill cursors */
+    memcpy(scnt, sptr, sizeof(int) * (size_t) n_dslot);
+    for (int h = 0; h < n_hit; h++) {
+        const int f = hit.p[4 * h], ia = hit.p[4 * h + 1], ib = hit.p[4 * h + 2], is = hit.p[4 * h + 3];
+        int below = 0, hi = n; /* the new index: f less the removed factors before it */
+        while (below < hi) {
+            int mid = (below + hi) / 2;
+            if (idx[mid] < f)
+                below = mid + 1;
+            else
+                hi = mid;
+        }
+        const int nf_ = f - below;
+        double pts[6];
+        eval_point(s, graph, f, pts);
+        int dst[3] = { ia >= 0 ? pcnt[ia]++ : -1, ib >= 0 ? pcnt[ib]++ : -1, is >= 0 ? scnt[is]++ : -1 };
+        for (int j = 0; j < 3; j++)
+            if (dst[j] >= 0) {
+                ent_f[dst[j]] = nf_;
+                memcpy(ent_pts + 6 * (size_t) dst[j], pts, sizeof(pts));
+            }
+    }
+    for (int i = 0; i < n_dirty; i++)
+        lamv[i] = dirty[i] < s->lam_n ? s->lam : 0.0;
+
+    /* ---- compaction: graph, mirror (host and HBM), plan, prior table ---- */
+    DEV_OK(asam_step_begin(dev)); /* one upload flush and one synchronisation for the whole removal */
+    gctx_remove_factors(c, n, idx);
+    if (plan_remove_factors(pl, dev, n, idx) != 0)
+        asam_fatal("%s: %s %s", fn, g_error, asam_last_error());
+    {
+        int o = 0;
+        for (int i = 0, k = 0; i < s->n_pr; i++) {
+            while (k < n && idx[k] < s->pr_f[i])
+                k++;
+            if (k < n && idx[k] == s->pr_f[i])
+                continue;
+            s->pr_f[o] = s->pr_f[i] - k;
+            memmove(s->pr_st + 3 * (size_t) o, s->pr_st + 3 * (size_t) i, 3 * sizeof(double));
+            o++;
+        }
+        s->n_pr = o;
+    }
+    graph_splice(graph, n, factor_idx, idx, removed_out);
+    param->factor_num = F - n;
+    s->removed = 1;
+    c->remove_epoch++;
+    s->epoch = c->remove_epoch;
+
+    /* ---- rebuild, re-factor the root paths, solve ---- */
+    int *tasks = NULL, *nwait = NULL, *keep = NULL, ntasks = 0;
+    plan_refactor(pl, marked, n_marked, &tasks, &nwait, &keep, &ntasks);
+    if (g_record_steps)
+        rec_tasks(&s->rec, ntasks, tasks, nwait, keep);
+    int policy_escalate = 0;
+    if (s->policy) {
+        aprilsam_b200_step_cost_t cost;
+        memset(&cost, 0, sizeof(cost));
+        plan_work(pl, tasks, ntasks, &cost.step_work, &cost.step_fronts, &cost.batch_work, &cost.batch_fronts);
+        cost.naffected = tr->naffected;
+        cost.nnodes = N;
+        cost.start_over = tr->start_over;
+        policy_escalate = s->policy(&cost, s->policy_user) != 0;
+    }
+    if (param->show_timing)
+        stamp(&tp, "scan, mark paths, compact");
+    DEV_OK(asam_hessian_rebuild(dev, n_dirty, dirty, pptr, n_dslot, dslot, sptr, n_ent, ent_f, ent_pts, lamv));
+    DEV_OK(asam_factor(dev, ntasks, tasks, nwait, keep));
+    step_solve(param, s, marked, n_marked, ntasks, nwait, 1, 0, &tp);
+    free(tasks); free(nwait); free(keep);
+    free(idx); free(dirty); free(dslot); free(rm); free(pcnt); free(scnt); free(dprior); ivec_free(&hit);
+    free(pptr); free(sptr); free(ent_f); free(ent_pts); free(lamv);
+    if (policy_escalate)
+        tr->start_over = INT_MAX;
+    step_escalate(graph, param);
+    return 0;
 }
 
 /* ---- test-only accessors (tools/gpu_diag.py, tests/) ------------------------------------------ */
@@ -1338,6 +1888,11 @@ static solver_t *marginal_solver(april_graph_t *g, april_graph_cholesky_param_t 
     }
     if (!s->plan_valid) {
         asam_set_error("%s: the plan was dropped (aprilsam_b200_invalidate_plan); solve again first", fn);
+        return NULL;
+    }
+    if (s->epoch != s->gc->remove_epoch) {
+        asam_set_error("%s: factors were removed from this graph through another param since this one last solved it; "
+                       "solve with april_graph_cholesky first", fn);
         return NULL;
     }
     if (zarray_size(g->nodes) != s->plan.N || zarray_size(g->factors) != s->plan.n_factors ||

@@ -545,6 +545,42 @@ H_EXPORT int h_candidate_mahalanobis(hctx_t *h, int k, const int *a, const int *
 {
     return aprilsam_b200_candidate_mahalanobis(h->g, h->p, k, a, b, z, W, d2, cov9);
 }
+
+/* aprilsam_b200_remove_factors; keep = 1 hands the removed factors back and destroys them here (exercises both
+ * ownership paths) */
+H_EXPORT int h_remove_factors(hctx_t *h, int n, const int *idx, int keep)
+{
+    if (!keep)
+        return aprilsam_b200_remove_factors(h->g, h->p, n, idx, NULL);
+    april_graph_factor_t **out = calloc((size_t) (n > 0 ? n : 1), sizeof(*out));
+    int rc = aprilsam_b200_remove_factors(h->g, h->p, n, idx, out);
+    for (int k = 0; rc == 0 && k < n; k++)
+        out[k]->destroy(out[k]);
+    free(out);
+    return rc;
+}
+
+/* further params on the same graph, for the tests of several solvers of one graph: h_swap_param makes one the
+ * harness's param (every h_* call then goes through it) and returns the one it replaces */
+H_EXPORT void *h_param_create(hctx_t *h)
+{
+    april_graph_cholesky_param_t *p = calloc(1, sizeof(*p));
+    april_graph_cholesky_param_init(p);
+    p->delta_xy = h->p->delta_xy;
+    p->delta_theta = h->p->delta_theta;
+    p->nthreshold = h->p->nthreshold;
+    p->tikhanov = h->p->tikhanov;
+    return p;
+}
+
+H_EXPORT void h_param_destroy(void *p) { april_graph_cholesky_param_destory(p); }
+
+H_EXPORT void *h_swap_param(hctx_t *h, void *p)
+{
+    void *old = h->p;
+    h->p = p;
+    return old;
+}
 #endif
 
 /* april_graph_cholesky_inc_solver (aprilsam.h:276): the reference never reads idxs (aprilsam.c:578-597) */

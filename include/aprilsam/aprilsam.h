@@ -310,6 +310,36 @@ int aprilsam_b200_relative_covariance(april_graph_t *graph, april_graph_cholesky
 int aprilsam_b200_candidate_mahalanobis(april_graph_t *graph, april_graph_cholesky_param_t *param, int k, const int *a,
                                         const int *b, const double *z, const double *W, double *d2, double *cov9);
 
+/* ---- factor removal (extension) --------------------------------------------------------------------------------
+ * Take the n distinct factors factor_idx[] out of graph->factors; the others keep their order (later indices shift
+ * down).  removed_out == NULL: the removed factors are destroyed through their destroy hook; otherwise removed_out[k]
+ * receives factor factor_idx[k] and the caller owns it.
+ *
+ * If `param` has never solved `graph` (param->chol == NULL) this is the splice alone.  If it continues a batch or
+ * incremental solve of `graph`, the solution is updated as an incremental step would update it, without
+ * relinearising or re-ordering: the Hessian becomes the system of the remaining factors, each at its own evaluation
+ * point (the l_points for xyt factors; for a prior, the l_point if it was there at the last batch solve, else the
+ * state it was added at), plus the last batch's tikhanov on the poses that existed then; only the supernodes on the
+ * root paths of the removed factors' poses are re-factored; label_changed, naffected (counted as if the removed
+ * factors had been added by a step), the back-substitution rule (every pose when naffected > 5, otherwise the marked
+ * paths, state = l_point + x), start_over, the nthreshold escalation and the escalation policy behave as in a step.
+ * param->factor_num becomes F - n.  The elimination order and param->tr stay until the next batch solve, which
+ * re-plans and takes the reference order of the reduced graph.  april_graph_chi2 and the queries above then work on
+ * the reduced graph.
+ *
+ * Returns 0, or -1 with the reason in aprilsam_b200_last_error() and nothing changed (graph, param, device state) for:
+ * NULL arguments or n < 1; an index outside [0, F) or listed twice; poses or factors added since the last solve (call
+ * april_graph_cholesky_inc first); a plan dropped by aprilsam_b200_invalidate_plan; a sharded batch solve; a removal
+ * that would leave a pose created since the last batch solve without any remaining factor connecting it to a pose of
+ * that batch or to a prior (its pivot would be zero); a remaining factor on a removed factor's pose whose z / W /
+ * loss was edited and re-checked (april_graph_chi2) since the last batch solve, so that HBM no longer holds the
+ * values it was linearised with.
+ *
+ * Another param that solved the same graph no longer matches it: its next april_graph_cholesky re-plans, its
+ * april_graph_cholesky_inc does nothing and sets aprilsam_b200_last_error, and its queries return -1, until then. */
+int aprilsam_b200_remove_factors(april_graph_t *graph, april_graph_cholesky_param_t *param, int n, const int *factor_idx,
+                                 april_graph_factor_t **removed_out);
+
 /* Relinearisation / re-ordering policy of april_graph_cholesky_inc().  The reference escalates an
  * incremental step to a full batch solve when `start_over > nthreshold` (kept) and, as shipped, also
  * when the step took longer than a third of the last batch solve by the WALL CLOCK

@@ -59,7 +59,8 @@ int asam_device_count(void);
 int asam_reserve(asam_dev_t *d, int n_nodes, int n_factors, int n_slots, int n_sn, int64_t ipool_ints,
                  int64_t arena_doubles);
 
-/* Graph mirror.  Factors are append-only (reference API has no removal). */
+/* Graph mirror.  Factors are appended; a removal (aprilsam_b200_remove_factors) uploads the compacted records again
+ * from its first removed index on. */
 int asam_upload_factors(asam_dev_t *d, int first, int count, const int32_t *type, const int32_t *na,
                         const int32_t *nb, const double *z3, const double *W9);
 /* Losses of robust xyt factors (type 32): per factor one 16-byte record {loss code as a double, k}
@@ -82,6 +83,17 @@ int asam_upload_desc(asam_dev_t *d, int n, const int32_t *sn_ids, const asam_sn_
 int asam_hessian_reset(asam_dev_t *d, int n_nodes, int n_slots, int n_lambda, double lambda);
 /* Zero a range of newly created positions / slots (incremental growth, no lambda). */
 int asam_hessian_clear_range(asam_dev_t *d, int q_first, int q_count, int slot_first, int slot_count);
+
+/* Factor removal (k_hessian_rebuild): OVERWRITE Adiag[9p] and Bq[3p] of the n_pose dirty poses pose[i] with lam[i] on
+ * the diagonal plus the blocks of the entries [pose_ptr[i], pose_ptr[i+1]), and Aoff[9s] of the n_slot dirty slots
+ * slot[i] with the off-diagonal blocks of the entries [slot_ptr[i], slot_ptr[i+1]) (+0.0 for none).  Entry e is factor
+ * ent_f[e] of the HBM mirror, evaluated at ent_pts[6e..6e+6) (pose a, then pose b; a prior uses the first three), with
+ * the maths of k_linearize.  Sums run in a fixed order, without atomics: the same tables give the same bits; nothing
+ * outside the dirty sets is written.  Tables in host memory, uploaded with the queued uploads; may be recorded between
+ * asam_step_begin and asam_step_run. */
+int asam_hessian_rebuild(asam_dev_t *d, int n_pose, const int32_t *pose, const int32_t *pose_ptr, int n_slot,
+                         const int32_t *slot, const int32_t *slot_ptr, int n_ent, const int32_t *ent_f,
+                         const double *ent_pts, const double *lam);
 
 /* Kernel 1: linearise factors [f_first, f_first+f_count) and scatter J'WJ / J'Wr into
  * Adiag/Aoff/Bq (replaces xyt_factor_eval + the assembly loop: april_graph_xyt.c:62-124,
@@ -149,7 +161,7 @@ int asam_set_shard_schedule(asam_dev_t *d, const asam_shard_sched_t *sched /* NU
 int asam_backsolve(asam_dev_t *d, int ntasks, const int32_t *btasks, const int32_t *bfirst);
 int asam_backsolve_full(asam_dev_t *d);
 
-/* Between asam_step_begin and asam_step_run, asam_linearize / asam_factor* / asam_backsolve* only
+/* Between asam_step_begin and asam_step_run, asam_linearize / asam_hessian_rebuild / asam_factor* / asam_backsolve* only
  * record their launch; asam_step_run pushes every queued upload with one copy and then launches
  * the recorded kernels in order (one incremental step = one H2D transfer). */
 int asam_step_begin(asam_dev_t *d);
