@@ -77,6 +77,7 @@ def lib() -> C.CDLL:
     L.asam_dbg_factor_loss.argtypes = [C.c_void_p, C.c_int, _ip, _dp]
     L.asam_chi2.argtypes = [C.c_void_p, C.c_int, _dp]
     L.aprilsam_b200_remove_factors.argtypes = [C.c_void_p, C.c_void_p, C.c_int, _ip, C.c_void_p]
+    L.aprilsam_b200_relinearize_poses.argtypes = [C.c_void_p, C.c_void_p, C.c_int, _ip]
     L.asam_hessian_rebuild.argtypes = [C.c_void_p, C.c_int, _ip, _ip, C.c_int, _ip, _ip, C.c_int, _ip, _dp, _dp]
     L.asam_dbg_plan_refactor.argtypes = [C.c_void_p, _ip, C.c_int, _ip, _ip, _ip, C.c_int]
     L.asam_dbg_plan_remove_factors.argtypes = [C.c_void_p, C.c_int, _ip]

@@ -75,12 +75,16 @@ def _load(impl: str) -> C.CDLL:
     for name, args in (("h_marginal_cov", [C.c_void_p, C.c_int, _ip, _dp]),
                        ("h_relative_cov", [C.c_void_p, C.c_int, C.c_int, _dp]),
                        ("h_candidate_mahalanobis", [C.c_void_p, C.c_int, _ip, _ip, _dp, _dp, _dp, _dp]),
-                       ("h_remove_factors", [C.c_void_p, C.c_int, _ip, C.c_int])):
+                       ("h_remove_factors", [C.c_void_p, C.c_int, _ip, C.c_int]),
+                       ("h_relinearize_poses", [C.c_void_p, C.c_int, _ip])):
         if hasattr(lib, name):
             getattr(lib, name).argtypes = args
             getattr(lib, name).restype = C.c_int
     for name, args, res in (("h_param_create", [C.c_void_p], C.c_void_p), ("h_param_destroy", [C.c_void_p], None),
-                            ("h_swap_param", [C.c_void_p, C.c_void_p], C.c_void_p)):
+                            ("h_swap_param", [C.c_void_p, C.c_void_p], C.c_void_p),
+                            ("h_set_relin_in_place", [C.c_void_p, C.c_int], None),
+                            ("h_relin_stats", [C.c_void_p, _dp], None),
+                            ("h_get_linearized", [C.c_void_p, _ip, C.c_int], C.c_int)):
         if hasattr(lib, name):
             getattr(lib, name).argtypes = args
             getattr(lib, name).restype = res
@@ -281,6 +285,30 @@ class Harness:
         if self.lib.h_remove_factors(self.h, len(idx), _i(idx), int(keep)) != 0:
             raise RuntimeError(self.lib.aprilsam_b200_last_error().decode())
 
+    def relinearize_poses(self, ids=None) -> None:
+        """aprilsam_b200_relinearize_poses: relinearise the poses `ids` in place (l_point = state) and update the
+        solution like an incremental step.  ids None: the poses the tree has flagged, passing the tree's own list
+        (tr->linearized_nodes).  Not the node hook `relinearize(i)`.  Raises RuntimeError with the library's message
+        when it returns -1."""
+        if ids is None:
+            rc = self.lib.h_relinearize_poses(self.h, 0, None)
+        else:
+            ids = np.ascontiguousarray(ids, dtype=np.int32).reshape(-1)
+            rc = self.lib.h_relinearize_poses(self.h, len(ids), _i(ids))
+        if rc != 0:
+            raise RuntimeError(self.lib.aprilsam_b200_last_error().decode())
+
+    def set_relin_in_place(self, threshold: int) -> None:
+        """replay_to relinearises the flagged poses in place after every step that leaves start_over above
+        `threshold` (its time counts in the step's ms); a negative threshold (the default) turns it off."""
+        self.lib.h_set_relin_in_place(self.h, int(threshold))
+
+    def relin_stats(self) -> tuple[int, float]:
+        """(relinearisations replay_to made, their wall ms)."""
+        out = np.zeros(2, dtype=np.float64)
+        self.lib.h_relin_stats(self.h, _d(out))
+        return int(out[0]), float(out[1])
+
     def new_param(self) -> int:
         """A further april_graph_cholesky_param_t for this graph (same settings); swap it in with swap_param."""
         return self.lib.h_param_create(self.h)
@@ -413,6 +441,12 @@ class Harness:
     def tree_parents(self) -> np.ndarray:
         out = np.zeros(max(self.n_nodes, 1), dtype=np.int32)
         n = self.lib.h_get_tree_parents(self.h, _i(out), out.size)
+        return out[:n]
+
+    def linearized_nodes(self) -> np.ndarray:
+        """tr->linearized_nodes: the poses flagged since the last batch solve, in the order they were flagged."""
+        out = np.zeros(max(self.n_nodes, 1), dtype=np.int32)
+        n = self.lib.h_get_linearized(self.h, _i(out), out.size)
         return out[:n]
 
     def graph_ptr(self) -> int:

@@ -133,6 +133,7 @@ typedef struct gctx {
     unsigned char *fstale;
     int n_stale, all_stale;
     unsigned remove_epoch; /* aprilsam_b200_remove_factors calls on this graph (solvers that missed one are stale) */
+    unsigned relin_epoch;  /* aprilsam_b200_relinearize_poses calls on this graph (likewise) */
     int fcap;
     double *stage; /* host staging for poses */
     int stage_cap;
@@ -373,7 +374,12 @@ ASAM_API double april_graph_chi2(april_graph_t *g)
 }
 
 /* ---- what the last incremental call asked of the kernels (tests; asam_dbg_record_steps) ------------- */
-enum { STEP_NONE = 0, STEP_SMALL = 1, STEP_PRUNED = 2, STEP_FULL = 3, STEP_FALLBACK = 4, STEP_REMOVE = 5, STEP_REMOVE_FULL = 6 };
+/* a step solved over a pruned traversal records its kind (STEP_PRUNED, STEP_REMOVE, STEP_RELIN), over the full one that
+ * kind + 1 */
+enum {
+    STEP_NONE = 0, STEP_SMALL = 1, STEP_PRUNED = 2, STEP_FULL = 3, STEP_FALLBACK = 4, STEP_REMOVE = 5, STEP_REMOVE_FULL = 6,
+    STEP_RELIN = 7, STEP_RELIN_FULL = 8
+};
 
 typedef struct step_rec {
     int kind, escalated, ntasks, nbt;
@@ -441,7 +447,7 @@ typedef struct solver {
     double *pr_st;
     int n_pr, pr_cap;
     int removed;
-    unsigned epoch; /* gc->remove_epoch as of this solver's last call */
+    unsigned epoch, relin_epoch; /* gc->remove_epoch / gc->relin_epoch as of this solver's last call */
 } solver_t;
 
 /* policies set before the first batch solve wait here for their solver (param -> fn) */
@@ -498,6 +504,7 @@ static solver_t *solver_get(april_graph_t *g, april_graph_cholesky_param_t *para
         s->hdr.is_spd = 1;
         s->gc = gctx_get(g);
         s->epoch = s->gc->remove_epoch;
+        s->relin_epoch = s->gc->relin_epoch;
         pthread_mutex_lock(&g_ctx_lock);
         s->gc->refs++;
         for (pending_policy_t **pp = &g_pending_policy; *pp; pp = &(*pp)->next)
@@ -513,6 +520,17 @@ static solver_t *solver_get(april_graph_t *g, april_graph_cholesky_param_t *para
         param->chol = &s->hdr;
     }
     return s;
+}
+
+/* Why the Hessian and factor in HBM no longer describe what this solver last solved, or NULL: another param on the same
+ * graph removed factors or relinearised poses since */
+static const char *stale_reason(const solver_t *s)
+{
+    if (s->epoch != s->gc->remove_epoch)
+        return "factors were removed from this graph through another param since this one last solved it";
+    if (s->relin_epoch != s->gc->relin_epoch)
+        return "poses of this graph were relinearised in place through another param since this one last solved it";
+    return NULL;
 }
 
 ASAM_API void aprilsam_b200_set_escalation_policy(april_graph_cholesky_param_t *param, aprilsam_b200_escalation_fn fn,
@@ -730,10 +748,11 @@ ASAM_API void april_graph_cholesky(april_graph_t *graph, april_graph_cholesky_pa
         asam_set_timing(dev, 1);
         stamp(&tp, "begin");
     }
-    if (s->epoch != c->remove_epoch) { /* another solver removed factors: this plan may match the counts, not the graph */
+    if (stale_reason(s)) { /* another solver removed factors (this plan may match the counts, not the graph) or relinearised */
         s->plan_valid = 0;
         s->tree_fresh = 0;
         s->epoch = c->remove_epoch;
+        s->relin_epoch = c->relin_epoch;
     }
     int restarted = 0;
 restart:;
@@ -979,14 +998,15 @@ static void apply_solution(solver_t *s, search_tree_t *tr, const double *x, int 
 static void inc_general_fallback(april_graph_t *graph, april_graph_cholesky_param_t *param, solver_t *s, int N, int F,
                                  int F0);
 
-/* The solve of an incremental step or a removal (:563, :578-597), after its re-factorisation was recorded
- * (asam_step_begin ... asam_factor): naffected > 5 back-substitutes every pose, otherwise only the supernodes the
- * traversal visits (the marked poses and their children, closed under ancestors), each from its first wanted pose
- * (bfirst).  Runs the recorded step, downloads x with the factorisation status and applies the solution
- * (apply_solution).  A removal (removal = 1) never takes the one-launch k_step, which knows only the kernels of a step,
- * and leaves the step counters of the host profile alone.  stage_off: doubles of the staging area still in use. */
+/* The solve of an incremental step, a removal or an in-place relinearisation (:563, :578-597), after its
+ * re-factorisation was recorded (asam_step_begin ... asam_factor): naffected > 5 back-substitutes every pose, otherwise
+ * only the supernodes the traversal visits (the marked poses and their children, closed under ancestors), each from its
+ * first wanted pose (bfirst).  Runs the recorded step, downloads x with the factorisation status and applies the
+ * solution (apply_solution).  kind: STEP_PRUNED for april_graph_cholesky_inc, STEP_REMOVE / STEP_RELIN for the rebuild
+ * steps, which never take the one-launch k_step (it knows only the kernels of a step) and leave the step counters of
+ * the host profile alone.  stage_off: doubles of the staging area still in use. */
 static void step_solve(april_graph_cholesky_param_t *param, solver_t *s, const int *marked, int n_marked, int ntasks,
-                       const int *nwait, int removal, int stage_off, stamps_t *tp)
+                       const int *nwait, int kind, int stage_off, stamps_t *tp)
 {
     PROF_BEGIN();
     gctx_t *c = s->gc;
@@ -994,13 +1014,16 @@ static void step_solve(april_graph_cholesky_param_t *param, solver_t *s, const i
     const plan_t *pl = &s->plan;
     search_tree_t *tr = param->tr;
     const int N = pl->N;
-    const char *where = removal ? "aprilsam_b200_remove_factors" : "april_graph_cholesky_inc";
+    const int rebuild = kind != STEP_PRUNED;
+    const char *where = kind == STEP_REMOVE  ? "aprilsam_b200_remove_factors"
+                        : kind == STEP_RELIN ? "aprilsam_b200_relinearize_poses"
+                                             : "april_graph_cholesky_inc";
     double *x = solver_x(s, N);
     int qbase = 0;
     int fstatus = 0;
     if (tr->naffected > 5) {
         if (g_record_steps)
-            s->rec.kind = removal ? STEP_REMOVE_FULL : STEP_FULL;
+            s->rec.kind = kind + 1;
         DEV_OK(asam_backsolve_full(dev));
         DEV_OK(asam_step_run(dev));
         DEV_OK(asam_download_x_status(dev, 0, N, x, &fstatus));
@@ -1052,7 +1075,7 @@ static void step_solve(april_graph_cholesky_param_t *param, solver_t *s, const i
             bfirst[i] = jf[bt[i]] < pl->desc[bt[i]].cb ? jf[bt[i]] : 0;
         DEV_OK(asam_backsolve(dev, nbt, bt, bfirst));
         /* a handful of single-CTA fronts: the whole step in ONE launch, results through pinned memory */
-        int small = !removal && nbt <= ASAM_SMALL_MAX_BS && ntasks <= ASAM_SMALL_MAX_TASKS && asam_step_small_supported(dev);
+        int small = !rebuild && nbt <= ASAM_SMALL_MAX_BS && ntasks <= ASAM_SMALL_MAX_TASKS && asam_step_small_supported(dev);
         for (int t = 0; small && t < ntasks; t++)
             small = ((nwait[t] >> 24) & 0x7f) <= 1;
         if (small) {
@@ -1084,19 +1107,19 @@ static void step_solve(april_graph_cholesky_param_t *param, solver_t *s, const i
             DEV_OK(asam_download_x_status(dev, qbase, N - qbase, x, &fstatus));
         }
         if (g_record_steps) {
-            s->rec.kind = removal ? STEP_REMOVE : small ? STEP_SMALL : STEP_PRUNED;
+            s->rec.kind = small ? STEP_SMALL : kind;
             rec_bt(&s->rec, nbt, bt, bfirst);
         }
     }
-    if (!removal)
+    if (!rebuild)
         PROF_LAP(4);
     report_factor_status(s, fstatus, where);
-    if (!removal)
+    if (!rebuild)
         PROF_LAP(5);
     if (param->show_timing)
         stamp(tp, "H2D, kernels, D2H of solution");
     apply_solution(s, tr, x, qbase);
-    if (!removal) {
+    if (!rebuild) {
         PROF_LAP(6);
         if (tr->naffected > 5)
             g_prof[17] += 1;
@@ -1160,9 +1183,9 @@ ASAM_API void april_graph_cholesky_inc(april_graph_t *graph, april_graph_cholesk
     if (!param->chol)
         return;
     solver_t *s = solver_of(param);
-    if (s->gc->graph == graph && s->epoch != s->gc->remove_epoch) {
-        asam_set_error("april_graph_cholesky_inc: factors were removed from this graph through another param since this "
-                       "one last solved it; nothing was done (solve with april_graph_cholesky first)");
+    if (s->gc->graph == graph && stale_reason(s)) {
+        asam_set_error("april_graph_cholesky_inc: %s; nothing was done (solve with april_graph_cholesky first)",
+                       stale_reason(s));
         return;
     }
     if (param->factor_num == F)
@@ -1298,7 +1321,7 @@ ASAM_API void april_graph_cholesky_inc(april_graph_t *graph, april_graph_cholesk
     param->nreordering = N;
     PROF_LAP(3);
 
-    step_solve(param, s, marked, n_marked, ntasks, nwait, 0, 6 * nf, &tp);
+    step_solve(param, s, marked, n_marked, ntasks, nwait, STEP_PRUNED, 6 * nf, &tp);
     free(tasks);
     free(nwait);
     free(keep);
@@ -1573,6 +1596,210 @@ static int unanchored_pose(const solver_t *s, int N, int F, const unsigned char 
     return bad;
 }
 
+/* ---- rebuild steps: the second half of a removal and of an in-place relinearisation ------------------------------- */
+/* The Hessian entries a rebuild step overwrites and the factors they are summed from.  The caller names the dirty poses
+ * and slots (ascending, distinct); rebuild_scan finds every factor on them with one pass over the factor list (O(F)),
+ * rebuild_tables evaluates them, rebuild_step re-factors and solves. */
+typedef struct rebuild {
+    ivec_t dirty, dslot;
+    int *pcnt, *scnt;      /* factors per dirty pose / dirty slot */
+    unsigned char *dprior; /* per dirty pose: a prior sits on it */
+    ivec_t hit;            /* (f, dirty pose index of a or -1, of b or -1, dirty slot index or -1) per factor found */
+    int stale;             /* the first factor found whose mirror gctx_verify_factors re-uploaded since the last batch */
+    /* the tables of asam_hessian_rebuild: entries [pptr[i], pptr[i+1]) for dirty pose i, [sptr[j], sptr[j+1]) for
+     * dirty slot j (sptr[0] = pptr[n_dirty]), each a factor index and its evaluation points; lambda per dirty pose */
+    int *pptr, *sptr, *ent_f, n_ent;
+    double *ent_pts, *lamv;
+} rebuild_t;
+
+static void ivec_sort_unique(ivec_t *v)
+{
+    qsort(v->p, (size_t) v->n, sizeof(int), cmp_int_asc);
+    int w = 0;
+    for (int i = 0; i < v->n; i++)
+        if (i == 0 || v->p[i] != v->p[i - 1])
+            v->p[w++] = v->p[i];
+    v->n = w;
+}
+
+static void rebuild_free(rebuild_t *rb)
+{
+    ivec_free(&rb->dirty);
+    ivec_free(&rb->dslot);
+    ivec_free(&rb->hit);
+    free(rb->pcnt);
+    free(rb->scnt);
+    free(rb->dprior);
+    free(rb->pptr);
+    free(rb->sptr);
+    free(rb->ent_f);
+    free(rb->ent_pts);
+    free(rb->lamv);
+    memset(rb, 0, sizeof(*rb));
+}
+
+/* Per dirty pose and per dirty slot, its factors in index order, skipping those with rm[f] set (rm may be NULL) */
+static void rebuild_scan(rebuild_t *rb, const solver_t *s, int F, const unsigned char *rm)
+{
+    const gctx_t *c = s->gc;
+    const int *dirty = rb->dirty.p, *dslot = rb->dslot.p, n_dirty = rb->dirty.n, n_dslot = rb->dslot.n;
+    rb->pcnt = calloc((size_t) n_dirty + 1, sizeof(int));
+    rb->scnt = calloc((size_t) n_dslot + 1, sizeof(int));
+    rb->dprior = calloc((size_t) n_dirty + 1, 1);
+    rb->stale = -1;
+    for (int f = 0; f < F; f++) {
+        if (rm && rm[f])
+            continue;
+        int two = asam_two_pose_type(c->ftype[f]);
+        int ia = find_int(dirty, n_dirty, c->fa[f]), ib = two ? find_int(dirty, n_dirty, c->fb[f]) : -1;
+        if (ia < 0 && ib < 0)
+            continue;
+        int is = two && ia >= 0 && ib >= 0 ? find_int(dslot, n_dslot, s->plan.fslot[f]) : -1;
+        if (c->fstale[f] && rb->stale < 0)
+            rb->stale = f;
+        ivec_push(&rb->hit, f);
+        ivec_push(&rb->hit, ia);
+        ivec_push(&rb->hit, ib);
+        ivec_push(&rb->hit, is);
+        if (ia >= 0)
+            rb->pcnt[ia]++;
+        if (ib >= 0)
+            rb->pcnt[ib]++;
+        if (is >= 0)
+            rb->scnt[is]++;
+        if (!two)
+            rb->dprior[ia] = 1;
+    }
+}
+
+/* The tables, every factor found at its evaluation point now (eval_point).  An entry holds the factor's index once the
+ * n_rm factors rm_sorted[] (ascending) have left the list: the index after a removal's compaction. */
+static void rebuild_tables(rebuild_t *rb, const solver_t *s, april_graph_t *g, int n_rm, const int *rm_sorted)
+{
+    const int n_dirty = rb->dirty.n, n_dslot = rb->dslot.n, n_hit = rb->hit.n / 4;
+    int *pptr = malloc(sizeof(int) * ((size_t) n_dirty + 1)), *sptr = malloc(sizeof(int) * ((size_t) n_dslot + 1));
+    pptr[0] = 0;
+    for (int i = 0; i < n_dirty; i++)
+        pptr[i + 1] = pptr[i] + rb->pcnt[i];
+    sptr[0] = pptr[n_dirty];
+    for (int i = 0; i < n_dslot; i++)
+        sptr[i + 1] = sptr[i] + rb->scnt[i];
+    const int n_ent = sptr[n_dslot];
+    int *ent_f = malloc(sizeof(int) * ((size_t) n_ent + 1));
+    double *ent_pts = malloc(sizeof(double) * 6 * ((size_t) n_ent + 1));
+    double *lamv = malloc(sizeof(double) * ((size_t) n_dirty + 1));
+    int *pcur = rb->pcnt, *scur = rb->scnt; /* the counts become fill cursors */
+    memcpy(pcur, pptr, sizeof(int) * (size_t) n_dirty);
+    memcpy(scur, sptr, sizeof(int) * (size_t) n_dslot);
+    for (int h = 0; h < n_hit; h++) {
+        const int *e = rb->hit.p + 4 * h;
+        const int f = e[0], ia = e[1], ib = e[2], is = e[3];
+        int below = 0, hi = n_rm; /* f less the removed factors before it */
+        while (below < hi) {
+            int mid = (below + hi) / 2;
+            if (rm_sorted[mid] < f)
+                below = mid + 1;
+            else
+                hi = mid;
+        }
+        double pts[6];
+        eval_point(s, g, f, pts);
+        int dst[3] = { ia >= 0 ? pcur[ia]++ : -1, ib >= 0 ? pcur[ib]++ : -1, is >= 0 ? scur[is]++ : -1 };
+        for (int j = 0; j < 3; j++)
+            if (dst[j] >= 0) {
+                ent_f[dst[j]] = f - below;
+                memcpy(ent_pts + 6 * (size_t) dst[j], pts, sizeof(pts));
+            }
+    }
+    for (int i = 0; i < n_dirty; i++)
+        lamv[i] = rb->dirty.p[i] < s->lam_n ? s->lam : 0.0;
+    rb->pptr = pptr;
+    rb->sptr = sptr;
+    rb->ent_f = ent_f;
+    rb->ent_pts = ent_pts;
+    rb->lamv = lamv;
+    rb->n_ent = n_ent;
+}
+
+/* Re-factor and solve a rebuild step whose uploads are recorded since asam_step_begin: mark the root paths of the dirty
+ * poses as if factors had been added on them (:482-498), overwrite the dirty entries (asam_hessian_rebuild), re-factor
+ * the marked supernodes (plan_refactor), solve like a step (step_solve with kind STEP_REMOVE or STEP_RELIN), then the
+ * policy hook and the nthreshold escalation of a step. */
+static void rebuild_step(rebuild_t *rb, april_graph_t *graph, april_graph_cholesky_param_t *param, solver_t *s, int kind,
+                         stamps_t *tp)
+{
+    plan_t *pl = &s->plan;
+    search_tree_t *tr = param->tr;
+    const int N = pl->N;
+    int *marked = solver_scratch(s, 2 * N + 16) + N + 8; /* upper half: apply_solution uses the lower */
+    int n_marked = 0;
+    tr->naffected = 0;
+    for (int i = 0; i < rb->dirty.n; i++) {
+        search_tree_node_t *node = &tr->nodes[rb->dirty.p[i]];
+        while (!node->label_changed) {
+            node->label_changed = 1;
+            tr->naffected++;
+            marked[n_marked++] = (int) (node - tr->nodes);
+            if (node->parent != -1)
+                node = &tr->nodes[node->parent];
+            else
+                break;
+        }
+    }
+    int *tasks = NULL, *nwait = NULL, *keep = NULL, ntasks = 0;
+    plan_refactor(pl, marked, n_marked, &tasks, &nwait, &keep, &ntasks);
+    if (g_record_steps)
+        rec_tasks(&s->rec, ntasks, tasks, nwait, keep);
+    int policy_escalate = 0;
+    if (s->policy) {
+        aprilsam_b200_step_cost_t cost;
+        memset(&cost, 0, sizeof(cost));
+        plan_work(pl, tasks, ntasks, &cost.step_work, &cost.step_fronts, &cost.batch_work, &cost.batch_fronts);
+        cost.naffected = tr->naffected;
+        cost.nnodes = N;
+        cost.start_over = tr->start_over;
+        policy_escalate = s->policy(&cost, s->policy_user) != 0;
+    }
+    if (param->show_timing)
+        stamp(tp, "scan, mark paths, rebuild tables");
+    DEV_OK(asam_hessian_rebuild(s->gc->dev, rb->dirty.n, rb->dirty.p, rb->pptr, rb->dslot.n, rb->dslot.p, rb->sptr,
+                                rb->n_ent, rb->ent_f, rb->ent_pts, rb->lamv));
+    DEV_OK(asam_factor(s->gc->dev, ntasks, tasks, nwait, keep));
+    step_solve(param, s, marked, n_marked, ntasks, nwait, kind, 0, tp);
+    free(tasks);
+    free(nwait);
+    free(keep);
+    if (policy_escalate)
+        tr->start_over = INT_MAX;
+    step_escalate(graph, param);
+}
+
+/* What a rebuild step needs of the solver it continues, checked before anything changes: NULL, or why not (and *tail,
+ * the advice that follows it in the error text).  sharded: the text for a sharded batch solve. */
+static const char *rebuild_refusal(const solver_t *s, april_graph_cholesky_param_t *param, april_graph_t *graph,
+                                   const char *sharded, const char **tail)
+{
+    const gctx_t *c = s->gc;
+    const int N = zarray_size(graph->nodes), F = zarray_size(graph->factors);
+    *tail = "";
+    if (c->graph != graph)
+        return "param does not continue a solve of this graph";
+    if (!s->plan_valid)
+        return "the plan was dropped (aprilsam_b200_invalidate_plan); solve again first";
+    if (stale_reason(s)) {
+        *tail = "; solve with april_graph_cholesky first";
+        return stale_reason(s);
+    }
+    if (s->plan.world > 1)
+        return sharded;
+    if (!param->tr || N != s->plan.N || F != s->plan.n_factors || F != param->factor_num || F != c->nf_dev)
+        return "poses or factors were added since the last solve (call april_graph_cholesky_inc first)";
+    if (c->all_stale)
+        return "a factor was replaced since the last batch solve (its HBM mirror no longer matches the linearised "
+               "Hessian); solve with april_graph_cholesky first";
+    return NULL;
+}
+
 ASAM_API int aprilsam_b200_remove_factors(april_graph_t *graph, april_graph_cholesky_param_t *param, int n,
                                           const int *factor_idx, april_graph_factor_t **removed_out)
 {
@@ -1610,23 +1837,12 @@ ASAM_API int aprilsam_b200_remove_factors(april_graph_t *graph, april_graph_chol
     }
     solver_t *s = solver_of(param);
     gctx_t *c = s->gc;
-    const char *why = NULL;
-    if (c->graph != graph)
-        why = "param does not continue a solve of this graph";
-    else if (!s->plan_valid)
-        why = "the plan was dropped (aprilsam_b200_invalidate_plan); solve again first";
-    else if (s->epoch != c->remove_epoch)
-        why = "factors were removed from this graph through another param since this one last solved it; solve with "
-              "april_graph_cholesky first";
-    else if (s->plan.world > 1)
-        why = "the last batch solve was sharded over several GPUs; removal continues single-GPU solves only";
-    else if (!param->tr || N != s->plan.N || F != s->plan.n_factors || F != param->factor_num || F != c->nf_dev)
-        why = "poses or factors were added since the last solve (call april_graph_cholesky_inc first)";
-    else if (c->all_stale)
-        why = "a factor was replaced since the last batch solve (its HBM mirror no longer matches the linearised "
-              "Hessian); solve with april_graph_cholesky first";
+    const char *tail, *why = rebuild_refusal(
+                          s, param, graph,
+                          "the last batch solve was sharded over several GPUs; removal continues single-GPU solves only",
+                          &tail);
     if (why) {
-        asam_set_error("%s: %s", fn, why);
+        asam_set_error("%s: %s%s", fn, why, tail);
         free(idx);
         return -1;
     }
@@ -1634,71 +1850,34 @@ ASAM_API int aprilsam_b200_remove_factors(april_graph_t *graph, april_graph_chol
     /* ---- validation on the unchanged state: dirty poses and slots, the remaining factors on them ---- */
     plan_t *pl = &s->plan;
     double t_scan = prof_now();
-    int *dirty = malloc(sizeof(int) * 2 * (size_t) n), n_dirty = 0;
-    int *dslot = malloc(sizeof(int) * (size_t) n), n_dslot = 0;
+    rebuild_t rb = { 0 };
     for (int k = 0; k < n; k++) {
         int f = idx[k];
-        dirty[n_dirty++] = c->fa[f];
+        ivec_push(&rb.dirty, c->fa[f]);
         if (asam_two_pose_type(c->ftype[f])) {
-            dirty[n_dirty++] = c->fb[f];
-            dslot[n_dslot++] = pl->fslot[f];
+            ivec_push(&rb.dirty, c->fb[f]);
+            ivec_push(&rb.dslot, pl->fslot[f]);
         }
     }
-    qsort(dirty, (size_t) n_dirty, sizeof(int), cmp_int_asc);
-    qsort(dslot, (size_t) n_dslot, sizeof(int), cmp_int_asc);
-    int w = 0;
-    for (int i = 0; i < n_dirty; i++)
-        if (i == 0 || dirty[i] != dirty[i - 1])
-            dirty[w++] = dirty[i];
-    n_dirty = w;
-    w = 0;
-    for (int i = 0; i < n_dslot; i++)
-        if (i == 0 || dslot[i] != dslot[i - 1])
-            dslot[w++] = dslot[i];
-    n_dslot = w;
-    /* one scan of the factor list: per dirty pose and per dirty slot, its remaining factors in index order
-     * (entries hold the index AFTER compaction) */
+    ivec_sort_unique(&rb.dirty);
+    ivec_sort_unique(&rb.dslot);
     unsigned char *rm = calloc((size_t) F, 1);
     for (int k = 0; k < n; k++)
         rm[idx[k]] = 1;
-    int *pcnt = calloc((size_t) n_dirty + 1, sizeof(int)), *scnt = calloc((size_t) n_dslot + 1, sizeof(int));
-    unsigned char *dprior = calloc((size_t) n_dirty + 1, 1);
-    ivec_t hit = { 0 }; /* (f, pose index or -1, slot index or -1) triples */
-    int stale = -1;
-    for (int f = 0; f < F; f++) {
-        if (rm[f])
-            continue;
-        int two = asam_two_pose_type(c->ftype[f]);
-        int ia = find_int(dirty, n_dirty, c->fa[f]), ib = two ? find_int(dirty, n_dirty, c->fb[f]) : -1;
-        if (ia < 0 && ib < 0)
-            continue;
-        int is = two && ia >= 0 && ib >= 0 ? find_int(dslot, n_dslot, pl->fslot[f]) : -1;
-        if (c->fstale[f] && stale < 0)
-            stale = f;
-        ivec_push(&hit, f);
-        ivec_push(&hit, ia);
-        ivec_push(&hit, ib);
-        ivec_push(&hit, is);
-        if (ia >= 0)
-            pcnt[ia]++;
-        if (ib >= 0)
-            pcnt[ib]++;
-        if (is >= 0)
-            scnt[is]++;
-        if (!two)
-            dprior[ia] = 1;
-    }
-    int bad = stale < 0 ? unanchored_pose(s, N, F, rm, dirty, n_dirty, dprior) : -1;
+    rebuild_scan(&rb, s, F, rm);
+    int bad = rb.stale < 0 ? unanchored_pose(s, N, F, rm, rb.dirty.p, rb.dirty.n, rb.dprior) : -1;
     t_scan = prof_now() - t_scan;
-    if (stale >= 0 || bad >= 0) {
-        if (stale >= 0)
+    free(rm);
+    if (rb.stale >= 0 || bad >= 0) {
+        if (rb.stale >= 0)
             asam_set_error("%s: factor %d, which shares a pose with a removed factor, was edited since the last batch "
                            "solve (its HBM mirror no longer holds the values the Hessian was built from); solve with "
-                           "april_graph_cholesky first", fn, stale);
+                           "april_graph_cholesky first", fn, rb.stale);
         else
             asam_set_error("%s: pose %d would be left unconstrained: it was created after the last batch solve and no "
                            "remaining factor connects it to a pose of that batch or to a prior", fn, bad);
-        free(idx); free(dirty); free(dslot); free(rm); free(pcnt); free(scnt); free(dprior); ivec_free(&hit);
+        free(idx);
+        rebuild_free(&rb);
         return -1;
     }
 
@@ -1706,7 +1885,6 @@ ASAM_API int aprilsam_b200_remove_factors(april_graph_t *graph, april_graph_chol
     g_prof[22] += t_scan;
     g_prof[23] += 1;
     asam_dev_t *dev = c->dev;
-    search_tree_t *tr = param->tr;
     stamps_t tp = { .n = 0 };
     if (param->show_timing) {
         asam_set_timing(dev, 1);
@@ -1718,62 +1896,7 @@ ASAM_API int aprilsam_b200_remove_factors(april_graph_t *graph, april_graph_chol
         s->rec.escalated = 0;
         s->rec.ntasks = s->rec.nbt = 0;
     }
-    /* root paths of the removed factors' poses, as if they had been added by a step (:482-498) */
-    int *marked = solver_scratch(s, 2 * N + 16) + N + 8; /* upper half: apply_solution uses the lower */
-    int n_marked = 0;
-    tr->naffected = 0;
-    for (int k = 0; k < n; k++) {
-        int f = idx[k], ends[2] = { c->fa[f], c->fb[f] };
-        for (int z0 = 0; z0 < (asam_two_pose_type(c->ftype[f]) ? 2 : 1); z0++) {
-            search_tree_node_t *node = &tr->nodes[ends[z0]];
-            while (!node->label_changed) {
-                node->label_changed = 1;
-                tr->naffected++;
-                marked[n_marked++] = (int) (node - tr->nodes);
-                if (node->parent != -1)
-                    node = &tr->nodes[node->parent];
-                else
-                    break;
-            }
-        }
-    }
-    /* the rebuild tables (evaluation points read before the mirror moves) */
-    const int n_hit = hit.n / 4;
-    int *pptr = malloc(sizeof(int) * ((size_t) n_dirty + 1)), *sptr = malloc(sizeof(int) * ((size_t) n_dslot + 1));
-    pptr[0] = 0;
-    for (int i = 0; i < n_dirty; i++)
-        pptr[i + 1] = pptr[i] + pcnt[i];
-    sptr[0] = pptr[n_dirty];
-    for (int i = 0; i < n_dslot; i++)
-        sptr[i + 1] = sptr[i] + scnt[i];
-    const int n_ent = sptr[n_dslot];
-    int *ent_f = malloc(sizeof(int) * ((size_t) n_ent + 1));
-    double *ent_pts = malloc(sizeof(double) * 6 * ((size_t) n_ent + 1));
-    double *lamv = malloc(sizeof(double) * ((size_t) n_dirty + 1));
-    memcpy(pcnt, pptr, sizeof(int) * (size_t) n_dirty); /* fill cursors */
-    memcpy(scnt, sptr, sizeof(int) * (size_t) n_dslot);
-    for (int h = 0; h < n_hit; h++) {
-        const int f = hit.p[4 * h], ia = hit.p[4 * h + 1], ib = hit.p[4 * h + 2], is = hit.p[4 * h + 3];
-        int below = 0, hi = n; /* the new index: f less the removed factors before it */
-        while (below < hi) {
-            int mid = (below + hi) / 2;
-            if (idx[mid] < f)
-                below = mid + 1;
-            else
-                hi = mid;
-        }
-        const int nf_ = f - below;
-        double pts[6];
-        eval_point(s, graph, f, pts);
-        int dst[3] = { ia >= 0 ? pcnt[ia]++ : -1, ib >= 0 ? pcnt[ib]++ : -1, is >= 0 ? scnt[is]++ : -1 };
-        for (int j = 0; j < 3; j++)
-            if (dst[j] >= 0) {
-                ent_f[dst[j]] = nf_;
-                memcpy(ent_pts + 6 * (size_t) dst[j], pts, sizeof(pts));
-            }
-    }
-    for (int i = 0; i < n_dirty; i++)
-        lamv[i] = dirty[i] < s->lam_n ? s->lam : 0.0;
+    rebuild_tables(&rb, s, graph, n, idx); /* evaluation points read before the mirror moves */
 
     /* ---- compaction: graph, mirror (host and HBM), plan, prior table ---- */
     DEV_OK(asam_step_begin(dev)); /* one upload flush and one synchronisation for the whole removal */
@@ -1800,31 +1923,132 @@ ASAM_API int aprilsam_b200_remove_factors(april_graph_t *graph, april_graph_chol
     s->epoch = c->remove_epoch;
 
     /* ---- rebuild, re-factor the root paths, solve ---- */
-    int *tasks = NULL, *nwait = NULL, *keep = NULL, ntasks = 0;
-    plan_refactor(pl, marked, n_marked, &tasks, &nwait, &keep, &ntasks);
-    if (g_record_steps)
-        rec_tasks(&s->rec, ntasks, tasks, nwait, keep);
-    int policy_escalate = 0;
-    if (s->policy) {
-        aprilsam_b200_step_cost_t cost;
-        memset(&cost, 0, sizeof(cost));
-        plan_work(pl, tasks, ntasks, &cost.step_work, &cost.step_fronts, &cost.batch_work, &cost.batch_fronts);
-        cost.naffected = tr->naffected;
-        cost.nnodes = N;
-        cost.start_over = tr->start_over;
-        policy_escalate = s->policy(&cost, s->policy_user) != 0;
+    rebuild_step(&rb, graph, param, s, STEP_REMOVE, &tp);
+    free(idx);
+    rebuild_free(&rb);
+    return 0;
+}
+
+/* ---- in-place relinearisation (extension) ---------------------------------------------------------------------- */
+ASAM_API int aprilsam_b200_relinearize_poses(april_graph_t *graph, april_graph_cholesky_param_t *param, int n,
+                                             const int *nodes)
+{
+    const char *fn = "aprilsam_b200_relinearize_poses";
+    if (!graph || !param || !nodes || n < 1) {
+        asam_set_error("%s: NULL graph / param / nodes or n < 1", fn);
+        return -1;
     }
-    if (param->show_timing)
-        stamp(&tp, "scan, mark paths, compact");
-    DEV_OK(asam_hessian_rebuild(dev, n_dirty, dirty, pptr, n_dslot, dslot, sptr, n_ent, ent_f, ent_pts, lamv));
-    DEV_OK(asam_factor(dev, ntasks, tasks, nwait, keep));
-    step_solve(param, s, marked, n_marked, ntasks, nwait, 1, 0, &tp);
-    free(tasks); free(nwait); free(keep);
-    free(idx); free(dirty); free(dslot); free(rm); free(pcnt); free(scnt); free(dprior); ivec_free(&hit);
-    free(pptr); free(sptr); free(ent_f); free(ent_pts); free(lamv);
-    if (policy_escalate)
-        tr->start_over = INT_MAX;
-    step_escalate(graph, param);
+    const int N = zarray_size(graph->nodes), F = zarray_size(graph->factors);
+    /* a copy first: nodes may be param->tr->linearized_nodes, which this call edits */
+    int *P = malloc(sizeof(int) * (size_t) n);
+    memcpy(P, nodes, sizeof(int) * (size_t) n);
+    unsigned char *inP = calloc((size_t) N + 1, 1);
+    for (int k = 0; k < n; k++) {
+        int bad = P[k] < 0 || P[k] >= N;
+        if (bad)
+            asam_set_error("%s: pose id %d (entry %d) is not in [0, %d)", fn, P[k], k, N);
+        else if ((bad = inP[P[k]]))
+            asam_set_error("%s: pose id %d (entry %d) is listed twice", fn, P[k], k);
+        if (bad) {
+            free(P);
+            free(inP);
+            return -1;
+        }
+        inP[P[k]] = 1;
+    }
+    const char *tail = "", *why = "param does not continue a solve of this graph";
+    if (param->chol)
+        why = rebuild_refusal(solver_of(param), param, graph,
+                              "the last batch solve was sharded over several GPUs; relinearisation in place continues "
+                              "single-GPU solves only", &tail);
+    if (why) {
+        asam_set_error("%s: %s%s", fn, why, tail);
+        free(P);
+        free(inP);
+        return -1;
+    }
+    solver_t *s = solver_of(param);
+    gctx_t *c = s->gc;
+    plan_t *pl = &s->plan;
+
+    /* ---- validation on the unchanged state: R = the factors with a pose in P; D = their poses and P; the dirty slots
+     * = the slots of R's two-pose factors; then every factor on D ---- */
+    double t_scan = prof_now();
+    rebuild_t rb = { 0 };
+    for (int k = 0; k < n; k++)
+        ivec_push(&rb.dirty, P[k]);
+    for (int f = 0; f < F; f++) {
+        if (asam_two_pose_type(c->ftype[f])) {
+            if (inP[c->fa[f]] || inP[c->fb[f]]) {
+                ivec_push(&rb.dirty, c->fa[f]);
+                ivec_push(&rb.dirty, c->fb[f]);
+                ivec_push(&rb.dslot, pl->fslot[f]);
+            }
+        }
+    }
+    ivec_sort_unique(&rb.dirty);
+    ivec_sort_unique(&rb.dslot);
+    rebuild_scan(&rb, s, F, NULL);
+    t_scan = prof_now() - t_scan;
+    if (rb.stale >= 0) {
+        asam_set_error("%s: factor %d, on a pose whose blocks the relinearisation rebuilds, was edited since the last "
+                       "batch solve (its HBM mirror no longer holds the values the Hessian was built from); solve with "
+                       "april_graph_cholesky first", fn, rb.stale);
+        free(P);
+        free(inP);
+        rebuild_free(&rb);
+        return -1;
+    }
+
+    /* ---- from here on the relinearisation happens ---- */
+    g_prof[22] += t_scan;
+    g_prof[23] += 1;
+    asam_dev_t *dev = c->dev;
+    search_tree_t *tr = param->tr;
+    stamps_t tp = { .n = 0 };
+    if (param->show_timing) {
+        asam_set_timing(dev, 1);
+        stamp(&tp, "begin");
+    }
+    s->tree_fresh = 0;
+    if (g_record_steps) {
+        s->rec.kind = STEP_NONE;
+        s->rec.escalated = 0;
+        s->rec.ntasks = s->rec.nbt = 0;
+    }
+    /* counters: the poses of P that were flagged are flagged no more */
+    int cleared = 0;
+    for (int k = 0; k < n; k++)
+        if (tr->nodes[P[k]].label_relinearized) {
+            tr->nodes[P[k]].label_relinearized = 0;
+            cleared++;
+        }
+    if (cleared) {
+        int w = 0;
+        for (int i = 0; i < tr->nlinearized_nodes; i++)
+            if (!inP[tr->linearized_nodes[i]])
+                tr->linearized_nodes[w++] = tr->linearized_nodes[i];
+        tr->nlinearized_nodes = w;
+        tr->start_over -= cleared;
+    }
+    /* l_point = state (the batch's copy, :131-135); a prior a step added on a pose of P moves with it */
+    for (int k = 0; k < n; k++) {
+        april_graph_node_t *nd = node_at(graph, P[k]);
+        memcpy(nd->l_point, nd->state, 3 * sizeof(double));
+    }
+    for (int i = 0; i < s->n_pr; i++)
+        if (inP[c->fa[s->pr_f[i]]])
+            memcpy(s->pr_st + 3 * (size_t) i, node_at(graph, c->fa[s->pr_f[i]])->l_point, 3 * sizeof(double));
+    rebuild_tables(&rb, s, graph, 0, NULL);
+    c->relin_epoch++;
+    s->relin_epoch = c->relin_epoch;
+
+    /* ---- rebuild, re-factor the root paths, solve ---- */
+    DEV_OK(asam_step_begin(dev)); /* one upload flush and one synchronisation */
+    rebuild_step(&rb, graph, param, s, STEP_RELIN, &tp);
+    free(P);
+    free(inP);
+    rebuild_free(&rb);
     return 0;
 }
 
@@ -1890,9 +2114,8 @@ static solver_t *marginal_solver(april_graph_t *g, april_graph_cholesky_param_t 
         asam_set_error("%s: the plan was dropped (aprilsam_b200_invalidate_plan); solve again first", fn);
         return NULL;
     }
-    if (s->epoch != s->gc->remove_epoch) {
-        asam_set_error("%s: factors were removed from this graph through another param since this one last solved it; "
-                       "solve with april_graph_cholesky first", fn);
+    if (stale_reason(s)) {
+        asam_set_error("%s: %s; solve with april_graph_cholesky first", fn, stale_reason(s));
         return NULL;
     }
     if (zarray_size(g->nodes) != s->plan.N || zarray_size(g->factors) != s->plan.n_factors ||

@@ -2,7 +2,7 @@
  *
  *   asam_replay --datapath FILE [--batch_update_only] [--delta_xy 0.1] [--delta_theta 0.1]
  *               [--nthreshold 100] [--quiet] [--show_timing] [--save OUT.graph]
- *               [--robust huber:K | cauchy:K]
+ *               [--robust huber:K | cauchy:K] [--relin-in-place N]
  *
  * FILE is a Manhattan-style text file (VERTEX2 id x y theta / EDGE2 a b dx dy dth I11 I12 I22 I33
  * I13 I23) or a ".graph" file in the stype framing.  The graph is then replayed pose by pose with
@@ -11,9 +11,11 @@
  * april_graph_cholesky, every later step april_graph_cholesky_inc (or the batch call with
  * --batch_update_only); chi2 and the step time are printed per step.  --robust creates every "scan" factor
  * (a loop closure, |a - b| != 1) as a robust xyt factor with a Huber or Cauchy loss of scale K > 0, so that
- * a wrong closure cannot pull the trajectory towards it.
- * Written against include/aprilsam/aprilsam.h only: without --robust (an aprilsam_b200 extension) it links
- * unchanged against the reference too.
+ * a wrong closure cannot pull the trajectory towards it.  --relin-in-place N relinearises the poses the tree has
+ * flagged (tr->linearized_nodes) in place, as one step, after every step that leaves start_over above N; combine it
+ * with a high --nthreshold so that the batch escalation does not come first.
+ * Written against include/aprilsam/aprilsam.h only: without --robust and --relin-in-place (aprilsam_b200
+ * extensions) it links unchanged against the reference too.
  */
 #define _POSIX_C_SOURCE 200809L
 #include <math.h>
@@ -102,7 +104,7 @@ static int parse_robust(const char *s, int *loss, double *k)
 int main(int argc, char **argv)
 {
     const char *path = NULL, *save = NULL;
-    int batch_only = 0, quiet = 0, nthreshold = 100, show_timing = 0, robust_loss = 0;
+    int batch_only = 0, quiet = 0, nthreshold = 100, show_timing = 0, robust_loss = 0, relin_in_place = -1;
     double delta_xy = 0.1, delta_theta = 0.1, robust_k = 0.0;
     for (int i = 1; i < argc; i++) {
         if (!strcmp(argv[i], "--robust")) {
@@ -121,9 +123,12 @@ int main(int argc, char **argv)
         else if (!strcmp(argv[i], "--delta_xy") && i + 1 < argc) delta_xy = atof(argv[++i]);
         else if (!strcmp(argv[i], "--delta_theta") && i + 1 < argc) delta_theta = atof(argv[++i]);
         else if (!strcmp(argv[i], "--nthreshold") && i + 1 < argc) nthreshold = atoi(argv[++i]);
+        else if (!strcmp(argv[i], "--relin-in-place") && i + 1 < argc && atoi(argv[i + 1]) >= 0)
+            relin_in_place = atoi(argv[++i]);
         else {
             fprintf(stderr, "usage: %s --datapath FILE [--batch_update_only] [--delta_xy D] [--delta_theta D] "
-                            "[--nthreshold N] [--quiet] [--save OUT.graph] [--robust huber:K | cauchy:K]\n", argv[0]);
+                            "[--nthreshold N] [--quiet] [--save OUT.graph] [--robust huber:K | cauchy:K] "
+                            "[--relin-in-place N]\n", argv[0]);
             return 2;
         }
     }
@@ -174,6 +179,7 @@ int main(int argc, char **argv)
     param->nthreshold = nthreshold;
     param->show_timing = show_timing; /* per-phase table after every solve (aprilsam.c:317) */
     double total = 0.0;
+    int relins = 0;
     for (int k = 0; k < N; k++) {
         april_graph_node_t *src;
         zarray_get(all->nodes, k, &src);
@@ -220,12 +226,22 @@ int main(int argc, char **argv)
             april_graph_cholesky(g, param);
         else
             april_graph_cholesky_inc(g, param);
+        if (relin_in_place >= 0 && k > 0 && !batch_only && param->tr->start_over > relin_in_place &&
+            param->tr->nlinearized_nodes > 0) {
+            if (aprilsam_b200_relinearize_poses(g, param, param->tr->nlinearized_nodes, param->tr->linearized_nodes)) {
+                fprintf(stderr, "step %d: %s\n", k, aprilsam_b200_last_error());
+                return 1;
+            }
+            relins++;
+        }
         double dt = now_ms() - t0;
         total += dt;
         if (!quiet)
             printf("step %d: chi2 %.6f, %.3f ms (total %.1f ms)\n", k, april_graph_chi2(g), dt, total);
     }
     printf("final chi2 %.9f after %d steps, solver time %.1f ms\n", april_graph_chi2(g), N, total);
+    if (relin_in_place >= 0)
+        printf("%d in-place relinearisations\n", relins);
     april_graph_cholesky_param_destory(param);
     april_graph_destroy(g);
     april_graph_destroy(all);

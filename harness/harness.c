@@ -38,6 +38,10 @@ typedef struct hctx {
     /* loss / k of the robust factors h_replay and h_load_full create for "scan" edges (0: plain xyt) */
     int scan_loss;
     double scan_k;
+    /* h_replay relinearises the flagged poses in place after a step whose start_over exceeds this (< 0: never) */
+    int relin_threshold;
+    int relin_calls;   /* those relinearisations so far, and their wall time */
+    double relin_ms;
 } hctx_t;
 
 static double now_ms(void)
@@ -66,6 +70,7 @@ H_EXPORT hctx_t *h_create(double delta_xy, double delta_theta, int nthreshold)
     h->p->delta_xy = delta_xy;
     h->p->delta_theta = delta_theta;
     h->p->nthreshold = nthreshold;
+    h->relin_threshold = -1;
     return h;
 }
 
@@ -234,6 +239,17 @@ H_EXPORT void h_info(hctx_t *h, int *info)
     info[6] = h->p->factor_num;
 }
 
+/* tr->linearized_nodes (the poses flagged since the last batch, in flag order); returns how many */
+H_EXPORT int h_get_linearized(hctx_t *h, int *out, int cap)
+{
+    search_tree_t *tr = h->p->tr;
+    if (!tr)
+        return 0;
+    int n = tr->nlinearized_nodes < cap ? tr->nlinearized_nodes : cap;
+    memcpy(out, tr->linearized_nodes, (size_t) (n > 0 ? n : 0) * sizeof(int));
+    return n;
+}
+
 /* elimination ordering of the last batch/inc call: out[pos] = graph node id */
 H_EXPORT int h_get_ordering(hctx_t *h, int *out, int cap)
 {
@@ -319,6 +335,20 @@ H_EXPORT int h_replay(hctx_t *h, int N, const double *init, const int *estart, c
             ms = h_batch(h);
         else
             ms = h_inc(h);
+#ifndef HARNESS_REFERENCE
+        if (h->relin_threshold >= 0 && k > 0 && !batch_only && h->p->tr && h->p->tr->start_over > h->relin_threshold &&
+            h->p->tr->nlinearized_nodes > 0) {
+            double t0 = now_ms();
+            if (aprilsam_b200_relinearize_poses(h->g, h->p, h->p->tr->nlinearized_nodes, h->p->tr->linearized_nodes)) {
+                fprintf(stderr, "harness: %s\n", aprilsam_b200_last_error());
+                abort();
+            }
+            double t = now_ms() - t0;
+            h->relin_calls++;
+            h->relin_ms += t;
+            ms += t;
+        }
+#endif
         if (ms_out)
             ms_out[done] = ms;
         if (chi2_out)
@@ -558,6 +588,29 @@ H_EXPORT int h_remove_factors(hctx_t *h, int n, const int *idx, int keep)
         out[k]->destroy(out[k]);
     free(out);
     return rc;
+}
+
+/* aprilsam_b200_relinearize_poses; ids == NULL relinearises the poses the tree has flagged, passing
+ * p->tr->linearized_nodes itself (the aliasing case) */
+H_EXPORT int h_relinearize_poses(hctx_t *h, int n, const int *ids)
+{
+    if (!ids) {
+        if (!h->p->tr)
+            return aprilsam_b200_relinearize_poses(h->g, h->p, 0, NULL);
+        return aprilsam_b200_relinearize_poses(h->g, h->p, h->p->tr->nlinearized_nodes, h->p->tr->linearized_nodes);
+    }
+    return aprilsam_b200_relinearize_poses(h->g, h->p, n, ids);
+}
+
+/* threshold >= 0: h_replay relinearises the flagged poses in place after every step that leaves start_over above it
+ * (its time counts in the step's ms); < 0 (the default): never */
+H_EXPORT void h_set_relin_in_place(hctx_t *h, int threshold) { h->relin_threshold = threshold; }
+
+/* out[0] = relinearisations h_replay made, out[1] = their wall ms */
+H_EXPORT void h_relin_stats(hctx_t *h, double *out)
+{
+    out[0] = h->relin_calls;
+    out[1] = h->relin_ms;
 }
 
 /* further params on the same graph, for the tests of several solvers of one graph: h_swap_param makes one the

@@ -340,6 +340,38 @@ int aprilsam_b200_candidate_mahalanobis(april_graph_t *graph, april_graph_choles
 int aprilsam_b200_remove_factors(april_graph_t *graph, april_graph_cholesky_param_t *param, int n, const int *factor_idx,
                                  april_graph_factor_t **removed_out);
 
+/* ---- in-place relinearisation (extension) --------------------------------------------------------------------------
+ * Relinearise the n distinct poses nodes[] (the set P) of a solved graph as one incremental step, without a batch
+ * solve, a new ordering or a new plan -- what an incremental smoother does about drift instead of starting over.
+ *
+ * For every pose p of P, l_point = state (the copy april_graph_cholesky makes); no other l_point changes.  R is every
+ * factor with a pose in P.  The dirty poses D are the poses of R's factors and P itself (a pose of P without factors
+ * holds only its lambda); the dirty slots are the slots of R's two-pose factors.  Afterwards each factor is evaluated
+ * where it was before (the l_points for xyt factors; for a prior, the l_point if it was there at the last batch solve,
+ * else the state it was added at), except that R's factors are evaluated at the new l_points of P: a prior added by a
+ * step on a pose of P moves to that pose's new l_point.  Every dirty pose is rebuilt from all its factors plus the last
+ * batch's tikhanov if the pose existed then, every dirty slot from all its factors (fixed-order overwrites on the GPU);
+ * nothing else in the Hessian is written.  The root paths of D are marked as if factors had been added on them
+ * (label_changed, naffected), only their supernodes are re-factored, and the solve is a step's: the back-substitution
+ * rule (every pose when naffected > 5, otherwise the marked paths, state = l_point + x), the escalation policy, the
+ * nthreshold escalation and start_over.  The elimination order, the plan, param->tr, param->factor_num and
+ * param->nreordering stay as they are.
+ *
+ * Counters, before the solve: every pose of P whose label_relinearized is set has it cleared and leaves
+ * tr->linearized_nodes (the other entries keep their order); nlinearized_nodes and start_over drop by that count;
+ * total_delta_xy / total_delta_theta stay.  The solve then flags poses as a step does, so a pose of P can be flagged
+ * again.  nodes may be param->tr->linearized_nodes itself with n = param->tr->nlinearized_nodes ("relinearise what the
+ * tree has flagged"): the list is copied before the tree is edited.
+ *
+ * Returns 0, or -1 with the reason in aprilsam_b200_last_error() and nothing changed (graph, param, device state) for:
+ * NULL arguments or n < 1; an id outside [0, N) or listed twice; a param that does not continue a solve of this graph;
+ * poses or factors added since the last solve (call april_graph_cholesky_inc first); a plan dropped by
+ * aprilsam_b200_invalidate_plan; a sharded batch solve; a factor replaced since the last batch solve; a factor on a
+ * dirty pose whose z / W / loss was edited and re-checked (april_graph_chi2) since the last batch solve, so that HBM no
+ * longer holds the values its other contributions were built from.  Another param that solved the same graph becomes
+ * stale as after a removal (its own error text names the relinearisation). */
+int aprilsam_b200_relinearize_poses(april_graph_t *graph, april_graph_cholesky_param_t *param, int n, const int *nodes);
+
 /* Relinearisation / re-ordering policy of april_graph_cholesky_inc().  The reference escalates an
  * incremental step to a full batch solve when `start_over > nthreshold` (kept) and, as shipped, also
  * when the step took longer than a third of the last batch solve by the WALL CLOCK
