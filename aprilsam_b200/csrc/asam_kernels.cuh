@@ -28,6 +28,7 @@
 #include <cstdint>
 
 #include "asam_cuda.h"
+#include "asam_loss.h"
 
 #define ASAM_TR_FLAG (1 << 30)
 #define ASAM_MAX_CACHED_CHILDREN 24
@@ -105,24 +106,6 @@ __device__ __forceinline__ void d_xyt_eval(const double *pa, const double *pb, c
 // Factor types (aprilsam.h): 1 xyt, 2 xytpos prior, 32 xyt with a robust loss.  Types 1 and 32 have the
 // same two poses, Jacobians and residual; the loss only scales W.
 __device__ __forceinline__ bool d_two_pose(const int type) { return type == 1 || type == 32; }
-
-// Robust loss of a type-32 factor at s = r'Wr (loss 1 Huber, 2 Cauchy; k > 0 and finite, checked on the
-// host): the IRLS weight w = rho'(s) and the cost rho(s).  A NaN s gives NaN for both.
-__device__ __forceinline__ double d_loss_weight(const int loss, const double k, const double s)
-{
-    const double k2 = k * k;
-    if (loss == 1)
-        return s <= k2 ? 1.0 : k / sqrt(s);
-    return 1.0 / (1.0 + s / k2);
-}
-
-__device__ __forceinline__ double d_loss_rho(const int loss, const double k, const double s)
-{
-    const double k2 = k * k;
-    if (loss == 1)
-        return s <= k2 ? s : 2.0 * k * sqrt(s) - k2;
-    return k2 * log1p(s / k2);
-}
 
 // 1/sqrt(a) for the Cholesky pivots: single-precision seed (MUFU.RSQ) + two Newton steps in double (relative
 // error 2^-22 -> 2^-43 -> below 2^-53; one to two ulp after rounding).  Three of these are CHAINED in every
@@ -267,7 +250,7 @@ __device__ __forceinline__ void linearize_body(const LinArgs &a, const int t)
             const double2 lk = a.f_loss[f];
             double X[3];
             d_av(W, r, X);
-            const double w = d_loss_weight((int) lk.x, lk.y, r[0] * X[0] + r[1] * X[1] + r[2] * X[2]);
+            const double w = asam_loss_weight((int) lk.x, lk.y, r[0] * X[0] + r[1] * X[1] + r[2] * X[2]);
 #pragma unroll
             for (int i = 0; i < 9; i++)
                 W[i] *= w;
@@ -423,7 +406,7 @@ __device__ __forceinline__ void rebuild_factor(const RebuildArgs &a, const int f
         const double2 lk = a.f_loss[f];
         double X[3];
         d_av(W, r, X);
-        const double w = d_loss_weight((int) lk.x, lk.y, r[0] * X[0] + r[1] * X[1] + r[2] * X[2]);
+        const double w = asam_loss_weight((int) lk.x, lk.y, r[0] * X[0] + r[1] * X[1] + r[2] * X[2]);
 #pragma unroll
         for (int i = 0; i < 9; i++)
             W[i] *= w;
@@ -2670,7 +2653,7 @@ __global__ void __launch_bounds__(256) k_chi2_partial(const int *f_type, const i
         const double s = r[0] * X[0] + r[1] * X[1] + r[2] * X[2];
         if (type == 32) { // robust xyt: 0.5 rho(s)
             const double2 lk = f_loss[f];
-            v = scale * d_loss_rho((int) lk.x, lk.y, s);
+            v = scale * asam_loss_rho((int) lk.x, lk.y, s);
         } else {
             v = scale * s;
         }

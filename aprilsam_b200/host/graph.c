@@ -18,6 +18,7 @@
 
 #include "aprilsam.h"
 #include "asam_host.h"
+#include "asam_loss.h"
 
 /* ---- matd (common/matd.h) ------------------------------------------------------------ */
 ASAM_API matd_t *matd_create(int rows, int cols)
@@ -324,18 +325,10 @@ void asam_factor_loss(const april_graph_factor_t *f, int32_t *loss, double *k)
 static april_graph_factor_eval_t *robust_weigh(const april_graph_factor_t *f, april_graph_factor_eval_t *ev)
 {
     const robust_loss_t *r = f->u.common.impl;
-    const double s = ev->chi2, k2 = r->k * r->k;
-    double w, rho;
-    if (r->loss == APRILSAM_B200_LOSS_HUBER) {
-        w = s <= k2 ? 1.0 : r->k / sqrt(s);
-        rho = s <= k2 ? s : 2.0 * r->k * sqrt(s) - k2;
-    } else {
-        w = 1.0 / (1.0 + s / k2);
-        rho = k2 * log1p(s / k2);
-    }
+    const double s = ev->chi2, w = asam_loss_weight(r->loss, r->k, s);
     for (int i = 0; i < 9; i++)
         ev->W->data[i] *= w;
-    ev->chi2 = rho;
+    ev->chi2 = asam_loss_rho(r->loss, r->k, s);
     return ev;
 }
 

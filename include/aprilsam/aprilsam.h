@@ -252,7 +252,10 @@ void aprilsam_b200_invalidate_plan(april_graph_cholesky_param_t *param);
  *   Cauchy  w = 1 / (1 + s / k^2)                   rho = k^2 log1p(s / k^2)
  * Every linearisation uses W_eff = w W (iteratively reweighted least squares, no second-order term);
  * april_graph_chi2 counts 0.5 rho(s) at the states.  The eval / state_eval hooks return W_eff and
- * chi2 = rho(s).  Files holding such factors ("april_graph_factor_xyt_robust") are this library's own. */
+ * chi2 = rho(s).  w and rho are accurate for every finite k > 0 and every finite s >= 0: within a few ulp of
+ * the exact value where that lies in [DBL_MIN, DBL_MAX / 4], within DBL_MIN of it below, never NaN.  So a
+ * Cauchy loss may be switched off with k = DBL_MAX, and a tiny k leaves a factor at zero residual its full W.
+ * Files holding such factors ("april_graph_factor_xyt_robust") are this library's own. */
 #define APRIL_GRAPH_FACTOR_XYT_ROBUST_TYPE 32
 enum { APRILSAM_B200_LOSS_HUBER = 1, APRILSAM_B200_LOSS_CAUCHY = 2 };
 /* NULL (text in aprilsam_b200_last_error) unless loss is one of the above and k is finite and > 0 */
