@@ -76,6 +76,13 @@ def lib() -> C.CDLL:
     L.asam_debug_marginal_pairs_layout.restype = None
     L.asam_dbg_factor_loss.argtypes = [C.c_void_p, C.c_int, _ip, _dp]
     L.asam_chi2.argtypes = [C.c_void_p, C.c_int, _dp]
+    L.aprilsam_b200_factor_residuals.argtypes = [C.c_void_p, C.c_int, C.c_int, _dp]
+    L.aprilsam_b200_factor_outlier_scores.argtypes = [C.c_void_p, C.c_void_p, C.c_int, _ip, _dp, _dp, _dp]
+    L.asam_factor_residuals.argtypes = [C.c_void_p, C.c_int, C.c_int, _dp]
+    L.asam_marginal_audit.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int,
+                                      C.c_void_p, _dp]
+    L.asam_debug_marginal_audit_layout.argtypes = [C.c_int, C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_int64)]
+    L.asam_debug_marginal_audit_layout.restype = None
     L.aprilsam_b200_remove_factors.argtypes = [C.c_void_p, C.c_void_p, C.c_int, _ip, C.c_void_p]
     L.aprilsam_b200_relinearize_poses.argtypes = [C.c_void_p, C.c_void_p, C.c_int, _ip]
     L.asam_hessian_rebuild.argtypes = [C.c_void_p, C.c_int, _ip, _ip, C.c_int, _ip, _ip, C.c_int, _ip, _dp, _dp]

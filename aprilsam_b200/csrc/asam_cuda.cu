@@ -99,7 +99,7 @@ struct asam_dev {
     int keep_off = 0; // ASAM_KEEP=0: always re-factor whole fronts (A/B measurements)
     // misc
     Buf ctrl;     // int[8]: [0] ticket, [1] err, [2] ticket backsolve
-    Buf partial;  // chi2 partial sums
+    Buf partial;  // chi2 partial sums; the output of asam_factor_residuals
     Buf patch_ids, patch_desc;
     Buf pts;
     Buf rb_int, rb_dbl; // tables of asam_hessian_rebuild
@@ -1458,6 +1458,24 @@ ASAM_EXPORT int asam_chi2(asam_dev_t *d, int n_factors, double *chi2_out)
     return download(d, chi2_out, partial, sizeof(double));
 }
 
+ASAM_EXPORT int asam_factor_residuals(asam_dev_t *d, int first, int count, double *out)
+{
+    if (first < 0 || count < 1 || !out)
+        return set_err("asam_factor_residuals: invalid arguments (first %d, count %d)", first, count);
+    CK(cudaSetDevice(d->device));
+    if (buf_reserve(d, d->partial, 6 * (size_t) count * sizeof(double), false, false))
+        return 1;
+    if (flush_uploads(d))
+        return 1;
+    k_factor_residuals<<<(count + 255) / 256, 256, 0, d->stream>>>(
+        (const int *) d->f_type.p, (const int *) d->f_a.p, (const int *) d->f_b.p, (const double *) d->f_z.p,
+        (const double *) d->f_W.p, (const double2 *) d->f_loss.p, (const double *) d->st.p, first, count,
+        (double *) d->partial.p);
+    d->n_launch += 1;
+    CK(cudaGetLastError());
+    return download(d, out, d->partial.p, 6 * (size_t) count * sizeof(double));
+}
+
 static size_t align256(size_t v) { return (v + 255) & ~(size_t) 255; }
 
 // Byte offsets in the query scratch: [err | out (3n x 3n)] [paths] [z] [hops]; err and out come back with one copy.
@@ -1495,6 +1513,26 @@ ASAM_EXPORT void asam_debug_marginal_pairs_layout(int n, int64_t z_doubles, int 
 {
     size_t o[6];
     marg_pairs_layout(n, z_doubles, n_hops, k, o);
+    for (int q = 0; q < 6; q++)
+        out6[q] = (int64_t) o[q];
+}
+
+// Byte offsets in the scratch of a factor audit: [err | out (11 doubles per factor)] [paths] [z] [hops] [records].
+// o = {out, paths, z, hops, records, total}.
+static void marg_audit_layout(int n, int64_t z_doubles, int n_hops, int k, size_t o[6])
+{
+    o[0] = 16;
+    o[1] = align256(o[0] + 11 * (size_t) k * sizeof(double));
+    o[2] = o[1] + align256((size_t) n * sizeof(asam_marg_path_t));
+    o[3] = o[2] + align256((size_t) z_doubles * sizeof(double));
+    o[4] = o[3] + align256(4 * (size_t) n_hops * sizeof(int));
+    o[5] = o[4] + align256((size_t) k * sizeof(asam_marg_audit_t));
+}
+
+ASAM_EXPORT void asam_debug_marginal_audit_layout(int n, int64_t z_doubles, int n_hops, int k, int64_t out6[6])
+{
+    size_t o[6];
+    marg_audit_layout(n, z_doubles, n_hops, k, o);
     for (int q = 0; q < 6; q++)
         out6[q] = (int64_t) o[q];
 }
@@ -1623,6 +1661,58 @@ ASAM_EXPORT int asam_marginal_pairs(asam_dev_t *d, int n, const asam_marg_path_t
         return set_err("asam_marginal_pairs: %s", err == 1 ? "a front on a path is larger than max_m"
                                                             : "a path's length differs from the plan's");
     memcpy(out, host.data() + 2, 10 * (size_t) k * sizeof(double));
+    return 0;
+}
+
+ASAM_EXPORT int asam_marginal_audit(asam_dev_t *d, int n, const asam_marg_path_t *paths, int64_t z_doubles,
+                                    int n_hops, int max_m, int k, const asam_marg_audit_t *recs, double *out)
+{
+    if (n < 1 || !paths || z_doubles < 3 || n_hops < n || max_m < 3 || k < 1 || !recs || !out)
+        return set_err("asam_marginal_audit: invalid arguments (n %d, z %lld, hops %d, max_m %d, k %d)", n,
+                       (long long) z_doubles, n_hops, max_m, k);
+    CK(cudaSetDevice(d->device));
+    const size_t smem = ASAM_MSMEM(max_m) * sizeof(double);
+    if (marg_smem_reserve(d->device, smem, max_m, "asam_marginal_audit"))
+        return 1;
+    size_t lay[6];
+    marg_audit_layout(n, z_doubles, n_hops, k, lay);
+    const size_t out_bytes = lay[0] + 11 * (size_t) k * sizeof(double);
+    if (buf_reserve(d, d->marg, lay[5], false, false))
+        return 1;
+    char *base = (char *) d->marg.p;
+    if (flush_uploads(d))
+        return 1;
+    CK(cudaMemcpyAsync(base + lay[1], paths, (size_t) n * sizeof(asam_marg_path_t), cudaMemcpyHostToDevice, d->stream));
+    CK(cudaMemcpyAsync(base + lay[4], recs, (size_t) k * sizeof(asam_marg_audit_t), cudaMemcpyHostToDevice, d->stream));
+    CK(cudaMemsetAsync(base, 0, 16, d->stream));
+    d->n_h2d += (int64_t) n * (int64_t) sizeof(asam_marg_path_t) + (int64_t) k * (int64_t) sizeof(asam_marg_audit_t);
+    MargArgs a;
+    a.sn = (const asam_sn_desc_t *) d->sn.p;
+    a.ipool = (const int *) d->ipool.p;
+    a.arena = (const double *) d->arena.p;
+    a.dinv = (const double *) d->dinv.p;
+    a.paths = (const asam_marg_path_t *) (base + lay[1]);
+    a.pairs = nullptr;
+    a.z = (double *) (base + lay[2]);
+    a.hop = (int *) (base + lay[3]);
+    a.out = (double *) (base + 16);
+    a.err = (int *) base;
+    a.n = n;
+    a.max_m = max_m;
+    k_marginal_path<<<n, 256, smem, d->stream>>>(a);
+    CK(cudaGetLastError());
+    k_marginal_audit<<<k, 128, 0, d->stream>>>(a, (const asam_marg_audit_t *) (base + lay[4]));
+    CK(cudaGetLastError());
+    d->n_launch += 2;
+    std::vector<double> host(out_bytes / sizeof(double));
+    if (download(d, host.data(), base, out_bytes))
+        return 1;
+    int err = 0;
+    memcpy(&err, host.data(), sizeof(int));
+    if (err)
+        return set_err("asam_marginal_audit: %s", err == 1 ? "a front on a path is larger than max_m"
+                                                            : "a path's length differs from the plan's");
+    memcpy(out, host.data() + 2, 11 * (size_t) k * sizeof(double));
     return 0;
 }
 

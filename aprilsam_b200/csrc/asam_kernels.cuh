@@ -2617,6 +2617,49 @@ __global__ void __launch_bounds__(256, 1) k_step(StepArgs a)
 // ------------------------------------------------------------------------------------------
 // chi2
 // ------------------------------------------------------------------------------------------
+// Factor f at the states: r (theta wrapped by mod2pi), s = r'Wr, and the term april_graph_chi2 adds for it (0.5 s,
+// 0.5 rho(s) for a robust factor, s for a prior) into v.  The same expressions as k_chi2_partial's lane, so that
+// k_factor_residuals' chi2 field is the exact value that lane adds (tests/test_gpu_audit.py checks the sums bit for
+// bit).  k_chi2_partial keeps its own copy: moved into this function it compiles to other SASS.
+__device__ __forceinline__ void d_chi2_term(const int *f_type, const int *f_a, const int *f_b, const double *f_z,
+                                            const double *f_W, const double2 *f_loss, const double *st, int f,
+                                            double r[3], double &s, double &v)
+{
+    int type = f_type[f];
+    int na = f_a[f];
+    double z[3], W[9];
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+        z[i] = f_z[3 * (size_t) f + i];
+#pragma unroll
+    for (int i = 0; i < 9; i++)
+        W[i] = f_W[9 * (size_t) f + i];
+    double scale;
+    if (d_two_pose(type)) { // xyt at `state`, weight 0.5   (april_graph.c:86-89)
+        int nb = f_b[f];
+        double pa[3], pb[3], Ja[9], Jb[9];
+#pragma unroll
+        for (int i = 0; i < 3; i++) { pa[i] = st[3 * (size_t) na + i]; pb[i] = st[3 * (size_t) nb + i]; }
+        d_xyt_eval(pa, pb, z, Ja, Jb, r);
+        scale = 0.5;
+    } else { // weight 1.0   (april_graph.c:90-93)
+        r[0] = z[0] - st[3 * (size_t) na + 0];
+        r[1] = z[1] - st[3 * (size_t) na + 1];
+        r[2] = d_mod2pi(z[2] - st[3 * (size_t) na + 2]);
+        scale = 1.0;
+    }
+    double X[3];
+    d_av(W, r, X);
+    const double sl = r[0] * X[0] + r[1] * X[1] + r[2] * X[2];
+    s = sl;
+    if (type == 32) { // robust xyt: 0.5 rho(s)
+        const double2 lk = f_loss[f];
+        v = scale * asam_loss_rho((int) lk.x, lk.y, sl);
+    } else {
+        v = scale * sl;
+    }
+}
+
 __global__ void __launch_bounds__(256) k_chi2_partial(const int *f_type, const int *f_a, const int *f_b,
                                                       const double *f_z, const double *f_W, const double2 *f_loss,
                                                       const double *st, int n_factors, double *partial)
@@ -2684,6 +2727,32 @@ __global__ void __launch_bounds__(256) k_chi2_final(const double *partial, int n
     }
     if (threadIdx.x == 0)
         out[0] = red[0];
+}
+
+// One thread per factor of [first, first + count): {r[3], s, w, chi2} (6 doubles), w the robust weight of a type-32
+// factor at s and 1 otherwise, chi2 the value k_chi2_partial's lane adds for the factor.
+__global__ void __launch_bounds__(256) k_factor_residuals(const int *f_type, const int *f_a, const int *f_b,
+                                                          const double *f_z, const double *f_W, const double2 *f_loss,
+                                                          const double *st, int first, int count, double *out)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count)
+        return;
+    const int f = first + i;
+    double r[3], s, v;
+    d_chi2_term(f_type, f_a, f_b, f_z, f_W, f_loss, st, f, r, s, v);
+    double w = 1.0;
+    if (f_type[f] == 32) {
+        const double2 lk = f_loss[f];
+        w = asam_loss_weight((int) lk.x, lk.y, s);
+    }
+    double *o = out + 6 * (size_t) i;
+    o[0] = r[0];
+    o[1] = r[1];
+    o[2] = r[2];
+    o[3] = s;
+    o[4] = w;
+    o[5] = v;
 }
 
 __global__ void k_apply_desc(asam_sn_desc_t *sn, const int *ids, const asam_sn_desc_t *desc, int n)
@@ -3042,4 +3111,119 @@ __global__ void __launch_bounds__(128) k_marginal_pairs(MargArgs a)
         d2 = (y0 * y0 + y1 * y1) + y2 * y2;
     }
     o[0] = d2;
+}
+
+// Sigma_aa, and for a closure Sigma_ab and Sigma_bb, by marg_block (each bit-identical to the block asam_marginal_cov
+// gives) into the caller's shared sg.  Called by all threads of a CTA; ends with a barrier.
+__device__ __forceinline__ void marg_sigma6(const MargArgs &a, int pa, int pb, double (*sg)[9])
+{
+    const int tid = threadIdx.x;
+    const asam_marg_path_t Pa = a.paths[pa];
+    double v = marg_block(a, Pa, Pa, true);
+    if (tid < 9)
+        sg[0][tid] = v;
+    if (pb >= 0) {
+        const asam_marg_path_t Pb = a.paths[pb];
+        v = marg_block(a, Pa, Pb, false);
+        if (tid < 9)
+            sg[1][tid] = v;
+        v = marg_block(a, Pb, Pb, true);
+        if (tid < 9)
+            sg[2][tid] = v;
+    }
+    __syncthreads();
+}
+
+// On one thread, from marg_sigma6's blocks: Sigma_rel = J Sigma_6 J' in the order of a row-major 3x6 by 6x6 by 6x3
+// product (symmetrised from its upper triangle; Sigma_aa itself for a prior, pb < 0): the expressions of
+// k_marginal_pairs, so that a factor's Sigma_rel is bit-identical to a candidate's on the same poses.  k_marginal_pairs
+// keeps its own copy: calling these helpers it compiles to other SASS.
+__device__ __forceinline__ void marg_rel(int pb, const double *J, const double (*sg)[9], double R[9])
+{
+    if (pb < 0) {
+#pragma unroll
+        for (int q = 0; q < 9; q++)
+            R[q] = sg[0][q];
+    } else {
+        // Sigma_6 = [S_aa S_ab; S_ab' S_bb], entry (k, c)
+        auto s6 = [&](int k, int c) -> double {
+            if (k < 3)
+                return c < 3 ? sg[0][3 * k + c] : sg[1][3 * k + c - 3];
+            return c < 3 ? sg[1][3 * c + k - 3] : sg[2][3 * (k - 3) + c - 3];
+        };
+        double JS[18];
+        for (int r = 0; r < 3; r++)
+            for (int c = 0; c < 6; c++) {
+                double acc = 0.0;
+                for (int k = 0; k < 6; k++)
+                    acc += J[6 * r + k] * s6(k, c);
+                JS[6 * r + c] = acc;
+            }
+        for (int r = 0; r < 3; r++)
+            for (int c = r; c < 3; c++) {
+                double acc = 0.0;
+                for (int k = 0; k < 6; k++)
+                    acc += JS[6 * r + k] * J[6 * c + k];
+                R[3 * r + c] = acc;
+                R[3 * c + r] = acc;
+            }
+    }
+}
+
+// One CTA per audited factor (asam_marg_audit_t): Sigma_rel by marg_rel (bit-identical to a candidate's on the same
+// poses), then on one thread, with W_f the information matrix the Hessian holds for the factor,
+//   N = W_f - W_f Sigma_rel W_f (symmetrised from its upper triangle), u = W_f r, N = L L', d2 = |L^-1 u|^2,
+//   redundancy = 3 - tr(Sigma_rel W_f).
+// d2 = r' (W_f^-1 - Sigma_rel)^-1 r where W_f is invertible: the candidate distance of the factor against the system
+// without it.  A pivot of N that is not > 0 (a bridge, a singular W_f) gives NaN.  out: 11 doubles per factor,
+// {d2, redundancy, Sigma_rel}; a factor's output depends only on its own record.
+__global__ void __launch_bounds__(128) k_marginal_audit(MargArgs a, const asam_marg_audit_t *rec)
+{
+    const asam_marg_audit_t &fr = rec[blockIdx.x];
+    const int pa = fr.pa, pb = fr.pb;
+    __shared__ double sg[3][9]; // Sigma_aa, Sigma_ab, Sigma_bb
+    marg_sigma6(a, pa, pb, sg);
+    if (threadIdx.x != 0)
+        return;
+    double R[9];
+    marg_rel(pb, fr.J, sg, R);
+    double W[9], T[9];
+#pragma unroll
+    for (int q = 0; q < 9; q++)
+        W[q] = fr.W[q];
+    // T = Sigma_rel W_f, N = W_f - W_f T
+#pragma unroll
+    for (int r = 0; r < 3; r++)
+#pragma unroll
+        for (int c = 0; c < 3; c++)
+            T[3 * r + c] = (R[3 * r] * W[c] + R[3 * r + 1] * W[3 + c]) + R[3 * r + 2] * W[6 + c];
+    double N[9];
+#pragma unroll
+    for (int r = 0; r < 3; r++)
+#pragma unroll
+        for (int c = r; c < 3; c++) {
+            const double v = W[3 * r + c] - ((W[3 * r] * T[c] + W[3 * r + 1] * T[3 + c]) + W[3 * r + 2] * T[6 + c]);
+            N[3 * r + c] = v;
+            N[3 * c + r] = v;
+        }
+    double u[3];
+#pragma unroll
+    for (int r = 0; r < 3; r++)
+        u[r] = (W[3 * r] * fr.r[0] + W[3 * r + 1] * fr.r[1]) + W[3 * r + 2] * fr.r[2];
+    const double l00 = N[0] > 0.0 ? sqrt(N[0]) : nan("");
+    const double l10 = N[3] / l00, l20 = N[6] / l00;
+    const double e11 = N[4] - l10 * l10;
+    const double l11 = e11 > 0.0 ? sqrt(e11) : nan("");
+    const double l21 = (N[7] - l20 * l10) / l11;
+    const double e22 = (N[8] - l20 * l20) - l21 * l21;
+    const double l22 = e22 > 0.0 ? sqrt(e22) : nan("");
+    const double y0 = u[0] / l00;
+    const double y1 = (u[1] - l10 * y0) / l11;
+    const double y2 = ((u[2] - l20 * y0) - l21 * y1) / l22;
+    double *o = a.out + 11 * (size_t) blockIdx.x;
+    o[0] = (y0 * y0 + y1 * y1) + y2 * y2;
+    o[1] = 3.0 - ((T[0] + T[4]) + T[8]);
+#pragma unroll
+    for (int q = 0; q < 9; q++)
+        o[2 + q] = R[q];
 }

@@ -75,6 +75,8 @@ def _load(impl: str) -> C.CDLL:
     for name, args in (("h_marginal_cov", [C.c_void_p, C.c_int, _ip, _dp]),
                        ("h_relative_cov", [C.c_void_p, C.c_int, C.c_int, _dp]),
                        ("h_candidate_mahalanobis", [C.c_void_p, C.c_int, _ip, _ip, _dp, _dp, _dp, _dp]),
+                       ("h_factor_residuals", [C.c_void_p, C.c_int, C.c_int, _dp]),
+                       ("h_factor_outlier_scores", [C.c_void_p, C.c_int, _ip, _dp, _dp, _dp]),
                        ("h_remove_factors", [C.c_void_p, C.c_int, _ip, C.c_int]),
                        ("h_relinearize_poses", [C.c_void_p, C.c_int, _ip])):
         if hasattr(lib, name):
@@ -276,6 +278,30 @@ class Harness:
                                             _d(cov) if with_cov else None) != 0:
             raise RuntimeError(self.lib.aprilsam_b200_last_error().decode())
         return (d2, cov) if with_cov else d2
+
+    def factor_residuals(self, first: int = 0, count=None):
+        """aprilsam_b200_factor_residuals: (count, 6) rows {r[0], r[1], r[2], s = r'Wr, w, chi2} of factors
+        [first, first + count) at the states (count None: up to the last factor).  Raises RuntimeError with the
+        library's message when it returns -1."""
+        if count is None:
+            count = max(self.n_factors - int(first), 0)
+        out = np.zeros((max(int(count), 1), 6), dtype=np.float64)
+        if self.lib.h_factor_residuals(self.h, int(first), int(count), _d(out)) != 0:
+            raise RuntimeError(self.lib.aprilsam_b200_last_error().decode())
+        return out[:int(count)]
+
+    def factor_outlier_scores(self, idx, with_cov: bool = False):
+        """aprilsam_b200_factor_outlier_scores: (d2, redundancy), each (k,), the leave-one-out Mahalanobis distances
+        and redundancies of factors idx against the last solve; with_cov also returns Sigma_rel (k x 3 x 3).  Raises
+        RuntimeError with the library's message when it returns -1."""
+        idx = np.ascontiguousarray(idx, dtype=np.int32).reshape(-1)
+        k = len(idx)
+        d2 = np.zeros(max(k, 1), dtype=np.float64)
+        red = np.zeros(max(k, 1), dtype=np.float64)
+        cov = np.zeros((max(k, 1), 3, 3), dtype=np.float64) if with_cov else None
+        if self.lib.h_factor_outlier_scores(self.h, k, _i(idx), _d(d2), _d(red), _d(cov) if with_cov else None) != 0:
+            raise RuntimeError(self.lib.aprilsam_b200_last_error().decode())
+        return (d2[:k], red[:k], cov[:k]) if with_cov else (d2[:k], red[:k])
 
     def remove_factors(self, idx, keep: bool = False) -> None:
         """aprilsam_b200_remove_factors: take factors idx out of the graph (the others keep their order) and update the

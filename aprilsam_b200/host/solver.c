@@ -27,6 +27,7 @@
 #include <time.h>
 
 #include "asam_host.h"
+#include "asam_loss.h"
 
 /* ---- errors -------------------------------------------------------------------------------- */
 static __thread char g_error[512];
@@ -297,6 +298,22 @@ static void gctx_sync_factors(gctx_t *c, april_graph_t *g)
  * 96-byte compare per factor and is run WHILE the kernels of the call are in flight (see
  * april_graph_cholesky): in the common case -- nothing changed -- it is free.
  * Returns 0 = unchanged, 1 = values re-uploaded, 2 = structure changed (mirror updated). */
+/* Factor i of the graph against mirror entry i: 0 same, 1 z / W / loss differ, 2 type or node ids differ (replaced) */
+static int factor_differs(const gctx_t *c, april_graph_t *g, int i)
+{
+    const april_graph_factor_t *f = factor_at(g, i);
+    const matd_t *Wm = f->u.common.W;
+    int na = f->nnodes > 0 ? f->nodes[0] : -1, nb = f->nnodes > 1 ? f->nodes[1] : -1;
+    if (f->type != c->ftype[i] || na != c->fa[i] || nb != c->fb[i] || !Wm || !f->u.common.z)
+        return 2;
+    const double *m = c->zw + 12 * (size_t) i;
+    int32_t loss;
+    double k;
+    asam_factor_loss(f, &loss, &k);
+    return memcmp(m, f->u.common.z, 3 * sizeof(double)) != 0 || memcmp(m + 3, Wm->data, 9 * sizeof(double)) != 0 ||
+           loss != c->floss[i] || memcmp(&k, &c->fk[i], sizeof(double)) != 0;
+}
+
 static int gctx_verify_factors(gctx_t *c, april_graph_t *g, int upto)
 {
     int changed = 0, structural = 0;
@@ -304,23 +321,17 @@ static int gctx_verify_factors(gctx_t *c, april_graph_t *g, int upto)
 #pragma omp parallel for schedule(static) reduction(| : changed, structural) reduction(min : lo) reduction(max : hi) \
     if (upto >= 4 * ASAM_OMP_MIN_NODES) num_threads(asam_host_threads())
     for (int i = 0; i < upto; i++) {
-        const april_graph_factor_t *f = factor_at(g, i);
-        const matd_t *Wm = f->u.common.W;
-        int na = f->nnodes > 0 ? f->nodes[0] : -1, nb = f->nnodes > 1 ? f->nodes[1] : -1;
-        if (f->type != c->ftype[i] || na != c->fa[i] || nb != c->fb[i] || !Wm || !f->u.common.z) {
+        const int d = factor_differs(c, g, i);
+        if (d == 2) {
             structural = 1;
             continue;
         }
-        double *m = c->zw + 12 * (size_t) i;
-        int32_t loss;
-        double k;
-        asam_factor_loss(f, &loss, &k);
-        if (memcmp(m, f->u.common.z, 3 * sizeof(double)) != 0 || memcmp(m + 3, Wm->data, 9 * sizeof(double)) != 0 ||
-            loss != c->floss[i] || memcmp(&k, &c->fk[i], sizeof(double)) != 0) {
+        if (d) {
+            const april_graph_factor_t *f = factor_at(g, i);
+            double *m = c->zw + 12 * (size_t) i;
             memcpy(m, f->u.common.z, 3 * sizeof(double));
-            memcpy(m + 3, Wm->data, 9 * sizeof(double));
-            c->floss[i] = loss;
-            c->fk[i] = k;
+            memcpy(m + 3, f->u.common.W->data, 9 * sizeof(double));
+            asam_factor_loss(f, &c->floss[i], &c->fk[i]);
             c->fstale[i] = 1;
             changed = 1;
             if (i < lo)
@@ -354,11 +365,10 @@ static int gctx_verify_factors(gctx_t *c, april_graph_t *g, int upto)
 }
 
 /* ---- chi2 (april_graph.c:79-98) -------------------------------------------------------------- */
-ASAM_API double april_graph_chi2(april_graph_t *g)
+/* The factor mirror checked and synced, the states uploaded: what the chi2 and residual kernels read */
+static gctx_t *gctx_for_states(april_graph_t *g)
 {
     int N = zarray_size(g->nodes), F = zarray_size(g->factors);
-    if (F == 0)
-        return 0.0;
     gctx_t *c = gctx_get(g);
     if (gctx_verify_factors(c, g, c->nf_dev < F ? c->nf_dev : F) == 2)
         c->nf_dev = 0; /* a factor was replaced: mirror everything again */
@@ -368,9 +378,36 @@ ASAM_API double april_graph_chi2(april_graph_t *g)
         memcpy(st + 3 * (size_t) i, node_at(g, i)->state, 3 * sizeof(double));
     DEV_OK(asam_reserve(c->dev, N + 64, 0, 0, 0, 0, 0));
     DEV_OK(asam_upload_points(c->dev, 1, 0, N, st));
+    return c;
+}
+
+ASAM_API double april_graph_chi2(april_graph_t *g)
+{
+    int F = zarray_size(g->factors);
+    if (F == 0)
+        return 0.0;
+    gctx_t *c = gctx_for_states(g);
     double chi2 = 0.0;
     DEV_OK(asam_chi2(c->dev, F, &chi2));
     return chi2;
+}
+
+/* ---- residuals of every factor (extension) --------------------------------------------------------- */
+ASAM_API int aprilsam_b200_factor_residuals(april_graph_t *g, int first, int count, aprilsam_b200_factor_residual_t *out)
+{
+    const char *fn = "aprilsam_b200_factor_residuals";
+    if (!g || !out) {
+        asam_set_error("%s: NULL graph or out", fn);
+        return -1;
+    }
+    const int F = zarray_size(g->factors);
+    if (first < 0 || count < 1 || first > F - count) {
+        asam_set_error("%s: factors [%d, %d + %d) are not a non-empty range of [0, %d)", fn, first, first, count, F);
+        return -1;
+    }
+    gctx_t *c = gctx_for_states(g);
+    DEV_OK(asam_factor_residuals(c->dev, first, count, (double *) out));
+    return 0;
 }
 
 /* ---- what the last incremental call asked of the kernels (tests; asam_dbg_record_steps) ------------- */
@@ -2219,17 +2256,18 @@ static int spd_inverse3(const double *W, double *Winv)
     return 1;
 }
 
-/* Sigma_rel (cov9, 9 doubles per candidate, may be NULL) and d2 of k candidates whose records hold J, r, Winv and
- * has_w (ids checked by the caller).  Runs the batches of plan_candidate_batches, one asam_marginal_pairs each. */
-static int candidates_run(solver_t *s, int k, const int *a, const int *b, asam_marg_pair_t *rec, double *d2,
-                          double *cov9, const char *fn)
+/* The batches of plan_candidate_batches over k records on poses a[c], b[c] (ids checked by the caller), one
+ * asam_marginal_pairs (pairs != NULL; 10 doubles per record into out) or asam_marginal_audit (audits != NULL; 11
+ * doubles per record) each.  Sets pa / pb of every record. */
+static int marginal_batches(solver_t *s, int k, const int *a, const int *b, asam_marg_pair_t *pairs,
+                            asam_marg_audit_t *audits, double *out, const char *fn)
 {
     const plan_t *pl = &s->plan;
+    const int stride = pairs ? 10 : 11;
     int *batch_end = malloc(sizeof(int) * (size_t) k), *pose_end = malloc(sizeof(int) * (size_t) k);
     int *poses = malloc(sizeof(int) * 2 * (size_t) k), *ia = malloc(sizeof(int) * (size_t) k);
     int *ib = malloc(sizeof(int) * (size_t) k);
     asam_marg_path_t *paths = malloc(sizeof(*paths) * 2 * (size_t) k);
-    double *out = malloc(sizeof(double) * 10 * (size_t) k);
     int nb = 0, rc = 0;
     plan_candidate_batches(pl, k, a, b, asam_candidate_budget / (int64_t) sizeof(double), batch_end, &nb, poses,
                            pose_end, ia, ib);
@@ -2246,18 +2284,19 @@ static int candidates_run(solver_t *s, int k, const int *a, const int *b, asam_m
             break;
         }
         for (int c = c0; c < c1; c++) {
-            rec[c].pa = ia[c];
-            rec[c].pb = ib[c];
+            if (pairs) {
+                pairs[c].pa = ia[c];
+                pairs[c].pb = ib[c];
+            } else {
+                audits[c].pa = ia[c];
+                audits[c].pb = ib[c];
+            }
         }
-        if (asam_marginal_pairs(s->gc->dev, n, paths, z, hops, pl->max_m, c1 - c0, rec + c0, out) != 0) {
+        double *o = out + (size_t) stride * (size_t) c0;
+        if ((pairs ? asam_marginal_pairs(s->gc->dev, n, paths, z, hops, pl->max_m, c1 - c0, pairs + c0, o)
+                   : asam_marginal_audit(s->gc->dev, n, paths, z, hops, pl->max_m, c1 - c0, audits + c0, o)) != 0) {
             asam_set_error("%s: %s", fn, asam_last_error());
             rc = -1;
-            break;
-        }
-        for (int c = c0; c < c1; c++) {
-            d2[c] = out[10 * (size_t) (c - c0)];
-            if (cov9)
-                memcpy(cov9 + 9 * (size_t) c, out + 10 * (size_t) (c - c0) + 1, 9 * sizeof(double));
         }
     }
     free(batch_end);
@@ -2266,6 +2305,21 @@ static int candidates_run(solver_t *s, int k, const int *a, const int *b, asam_m
     free(ia);
     free(ib);
     free(paths);
+    return rc;
+}
+
+/* Sigma_rel (cov9, 9 doubles per candidate, may be NULL) and d2 of k candidates whose records hold J, r, Winv and
+ * has_w (ids checked by the caller). */
+static int candidates_run(solver_t *s, int k, const int *a, const int *b, asam_marg_pair_t *rec, double *d2,
+                          double *cov9, const char *fn)
+{
+    double *out = malloc(sizeof(double) * 10 * (size_t) k);
+    int rc = marginal_batches(s, k, a, b, rec, NULL, out, fn);
+    for (int c = 0; c < k && rc == 0; c++) {
+        d2[c] = out[10 * (size_t) c];
+        if (cov9)
+            memcpy(cov9 + 9 * (size_t) c, out + 10 * (size_t) c + 1, 9 * sizeof(double));
+    }
     free(out);
     return rc;
 }
@@ -2342,4 +2396,87 @@ ASAM_API int aprilsam_b200_relative_covariance(april_graph_t *g, april_graph_cho
     candidate_jacobian(g, a, b, rec.J);
     double d2;
     return candidates_run(s, 1, &a, &b, &rec, &d2, out9, fn);
+}
+
+/* ---- factor audit: leave-one-out Mahalanobis distances and redundancies (extension) ---------------------------- */
+ASAM_API int aprilsam_b200_factor_outlier_scores(april_graph_t *g, april_graph_cholesky_param_t *param, int k,
+                                                 const int *factor_idx, double *d2, double *redundancy, double *cov9)
+{
+    const char *fn = "aprilsam_b200_factor_outlier_scores";
+    if (k < 1 || !factor_idx || !d2 || !redundancy) {
+        asam_set_error("%s: NULL factor_idx / d2 / redundancy or k < 1", fn);
+        return -1;
+    }
+    solver_t *s = marginal_solver(g, param, fn);
+    if (!s)
+        return -1;
+    const gctx_t *c = s->gc;
+    const int F = zarray_size(g->factors);
+    if (c->all_stale || c->nf_dev != F) {
+        asam_set_error("%s: a factor was replaced since the last batch solve (its HBM mirror no longer matches the "
+                       "linearised Hessian); solve with april_graph_cholesky first", fn);
+        return -1;
+    }
+    asam_marg_audit_t *rec = calloc((size_t) k, sizeof(*rec));
+    int *a = malloc(sizeof(int) * (size_t) k), *b = malloc(sizeof(int) * (size_t) k);
+    int rc = 0;
+    for (int q = 0; q < k && rc == 0; q++) {
+        const int f = factor_idx[q];
+        if (f < 0 || f >= F) {
+            asam_set_error("%s: entry %d: factor index %d is not in [0, %d)", fn, q, f, F);
+            rc = -1;
+            break;
+        }
+        const int d = factor_differs(c, g, f);
+        if (d == 2) {
+            asam_set_error("%s: entry %d: factor %d was replaced since the last solve; solve with april_graph_cholesky "
+                           "first", fn, q, f);
+            rc = -1;
+            break;
+        }
+        if (d || c->fstale[f]) {
+            asam_set_error("%s: entry %d: factor %d was edited since the last batch solve (z / W / loss differ from "
+                           "what the Hessian was built from); solve with april_graph_cholesky first", fn, q, f);
+            rc = -1;
+            break;
+        }
+        const int two = asam_two_pose_type(c->ftype[f]);
+        const double *z = c->zw + 12 * (size_t) f, *W = z + 3;
+        asam_marg_audit_t *r = rec + q;
+        a[q] = c->fa[f];
+        b[q] = two ? c->fb[f] : -1;
+        const double *sa = node_at(g, a[q])->state;
+        double w = 1.0;
+        if (two) {
+            candidate_jacobian(g, a[q], b[q], r->J);
+            asam_xyt_residual(z, sa, node_at(g, b[q])->state, r->r);
+            if (c->ftype[f] == APRIL_GRAPH_FACTOR_XYT_ROBUST_TYPE) { /* w at the evaluation point, as linearised */
+                double pts[6], re[3], X[3];
+                eval_point(s, g, f, pts);
+                asam_xyt_residual(z, pts, pts + 3, re);
+                for (int i = 0; i < 3; i++)
+                    X[i] = W[3 * i] * re[0] + W[3 * i + 1] * re[1] + W[3 * i + 2] * re[2];
+                w = asam_loss_weight(c->floss[f], c->fk[f], re[0] * X[0] + re[1] * X[1] + re[2] * X[2]);
+            }
+        } else {
+            asam_xytpos_residual(z, sa, r->r);
+        }
+        for (int i = 0; i < 9; i++)
+            r->W[i] = W[i] * w;
+    }
+    double *out = rc == 0 ? malloc(sizeof(double) * 11 * (size_t) k) : NULL;
+    if (rc == 0)
+        rc = marginal_batches(s, k, a, b, NULL, rec, out, fn);
+    for (int q = 0; q < k && rc == 0; q++) {
+        const double *o = out + 11 * (size_t) q;
+        d2[q] = o[0];
+        redundancy[q] = o[1];
+        if (cov9)
+            memcpy(cov9 + 9 * (size_t) q, o + 2, 9 * sizeof(double));
+    }
+    free(out);
+    free(rec);
+    free(a);
+    free(b);
+    return rc;
 }

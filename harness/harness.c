@@ -576,6 +576,17 @@ H_EXPORT int h_candidate_mahalanobis(hctx_t *h, int k, const int *a, const int *
     return aprilsam_b200_candidate_mahalanobis(h->g, h->p, k, a, b, z, W, d2, cov9);
 }
 
+/* aprilsam_b200_factor_residuals (out: 6 doubles per factor) / _factor_outlier_scores */
+H_EXPORT int h_factor_residuals(hctx_t *h, int first, int count, double *out)
+{
+    return aprilsam_b200_factor_residuals(h->g, first, count, (aprilsam_b200_factor_residual_t *) out);
+}
+
+H_EXPORT int h_factor_outlier_scores(hctx_t *h, int k, const int *idx, double *d2, double *redundancy, double *cov9)
+{
+    return aprilsam_b200_factor_outlier_scores(h->g, h->p, k, idx, d2, redundancy, cov9);
+}
+
 /* aprilsam_b200_remove_factors; keep = 1 hands the removed factors back and destroys them here (exercises both
  * ownership paths) */
 H_EXPORT int h_remove_factors(hctx_t *h, int n, const int *idx, int keep)

@@ -313,6 +313,56 @@ int aprilsam_b200_relative_covariance(april_graph_t *graph, april_graph_cholesky
 int aprilsam_b200_candidate_mahalanobis(april_graph_t *graph, april_graph_cholesky_param_t *param, int k, const int *a,
                                         const int *b, const double *z, const double *W, double *d2, double *cov9);
 
+/* ---- factor audit (extension) ------------------------------------------------------------------------------------
+ * Which accepted factor has proved false.  A raw residual is the wrong test: the solve pulls the graph towards an
+ * outlier, so its residual shrinks, and a factor the rest of the graph hardly checks looks good even when it is wrong.
+ *
+ * aprilsam_b200_factor_residuals: per factor f of [first, first + count), at the states (the values april_graph_chi2
+ * sees): r = z - h(state) (theta wrapped by mod2pi, as the eval hooks compute it), s = r'Wr, the robust weight
+ * w = w(s) of a robust factor (1 for other types) and chi2, the term april_graph_chi2 adds for f (0.5 s, 0.5 rho(s)
+ * for a robust factor, s for a prior).  Summed in april_graph_chi2's order (256-factor blocks, each a 256-lane tree,
+ * then a 256-lane tree over the blocks) the chi2 fields give april_graph_chi2 bit for bit.  Like april_graph_chi2 it
+ * needs no solve and no param: it checks the factors against their HBM mirror (re-uploading edits), uploads the
+ * states and runs one kernel.  Returns 0, or -1 with the reason in aprilsam_b200_last_error() for NULL arguments or a
+ * range that is empty or not inside [0, F). */
+typedef struct {
+    double r[3];
+    double s;
+    double w;
+    double chi2;
+} aprilsam_b200_factor_residual_t;
+int aprilsam_b200_factor_residuals(april_graph_t *graph, int first, int count, aprilsam_b200_factor_residual_t *out);
+
+/* aprilsam_b200_factor_outlier_scores: the leave-one-out test of k factors of a solved graph (indices factor_idx[],
+ * repeats allowed), with Sigma as aprilsam_b200_marginal_covariance defines it.  For factor f, with J = [J_a J_b] at
+ * its evaluation point (the l_points), r its residual at the states, W_f the information matrix the Hessian holds
+ * for it (W; w W for a robust factor, w at the evaluation point) and
+ *   Sigma_rel = J Sigma_ab J'  (an xyt factor: exactly aprilsam_b200_relative_covariance(a, b))
+ *   Sigma_rel = Sigma_aa       (a prior: the diagonal block of aprilsam_b200_marginal_covariance),
+ *   d2[q]         = (W_f r)' N^-1 (W_f r),  N = W_f - W_f Sigma_rel W_f  (= r' (W_f^-1 - Sigma_rel)^-1 r)
+ *   redundancy[q] = 3 - tr(Sigma_rel W_f).
+ * In the linear model d2 is exactly the candidate distance (aprilsam_b200_candidate_mahalanobis) the factor would get
+ * against the solve of the graph without it: compare it with a chi-square quantile with 3 degrees of freedom, for
+ * example 16.27 (99.9 %).  The redundancy, in [0, 3], is how much of the factor the rest of the graph checks; summed
+ * over all factors it gives the graph's degrees of freedom.  A bridge has redundancy 0 and cannot be tested: N is
+ * singular and d2 is NaN (as for a non-positive pivot of N).  A factor with little redundancy gives a weak test.
+ * r is taken at the states and J at the l_points: the test is the leave-one-out test of the linearised problem, so it
+ * describes outliers only near convergence.  After a single solve from a poor initial guess, correct factors can
+ * score high too; solve until the step is small before judging factors by d2.
+ *
+ * cov9 (NULL allowed): Sigma_rel, 9 doubles row-major.  A factor's outputs are the same alone or in any request, in
+ * any order and batch split, and from call to call; nothing but the query scratch on the GPU is written.  The cost
+ * follows the root paths of the factors' distinct poses: a pose near the leaves of a large graph has a long path, so
+ * score the loop closures that aprilsam_b200_factor_residuals flags, not every factor of a large graph.
+ *
+ * Returns 0, or -1 with the reason in aprilsam_b200_last_error() and nothing changed for the cases of the covariance
+ * queries above, and for k < 1, NULL factor_idx / d2 / redundancy, an index outside [0, F), a factor replaced since
+ * the last solve, or a factor whose z / W / loss differs from the values the Hessian was built from (edited since the
+ * last batch solve, whether or not april_graph_chi2 has re-checked it since); the message names the entry at
+ * fault.  d2, redundancy and cov9 are unspecified after an error; the solver stays usable. */
+int aprilsam_b200_factor_outlier_scores(april_graph_t *graph, april_graph_cholesky_param_t *param, int k,
+                                        const int *factor_idx, double *d2, double *redundancy, double *cov9);
+
 /* ---- factor removal (extension) --------------------------------------------------------------------------------
  * Take the n distinct factors factor_idx[] out of graph->factors; the others keep their order (later indices shift
  * down).  removed_out == NULL: the removed factors are destroyed through their destroy hook; otherwise removed_out[k]
@@ -404,6 +454,7 @@ int aprilsam_b200_policy_work_ratio(const aprilsam_b200_step_cost_t *cost, void 
 #if defined(__x86_64__) && !defined(__cplusplus)
 #include <stddef.h>
 _Static_assert(sizeof(zarray_t) == 24, "zarray_t");
+_Static_assert(sizeof(aprilsam_b200_factor_residual_t) == 6 * sizeof(double), "aprilsam_b200_factor_residual_t");
 _Static_assert(sizeof(april_graph_t) == 32, "april_graph_t");
 _Static_assert(sizeof(april_graph_node_t) == 112 && offsetof(april_graph_node_t, state) == 16 &&
                    offsetof(april_graph_node_t, l_point) == 40 && offsetof(april_graph_node_t, delta_X) == 48 &&

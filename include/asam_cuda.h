@@ -220,9 +220,30 @@ typedef struct asam_marg_pair {
 int asam_marginal_pairs(asam_dev_t *d, int n, const asam_marg_path_t *paths, int64_t z_doubles, int n_hops, int max_m,
                         int k, const asam_marg_pair_t *pairs, double *out);
 
+/* One factor of asam_marginal_audit: an xyt factor between the poses of paths[pa] and paths[pb], or a prior on
+ * paths[pa] (pb = -1).  J = [J_a J_b] (3 x 6, row-major) at the factor's evaluation point, r the residual at the
+ * states, W the information matrix the Hessian holds for it (w W for a robust factor, w at the evaluation point). */
+typedef struct asam_marg_audit {
+    int32_t pa, pb;
+    double J[18];
+    double r[3];
+    double W[9];
+} asam_marg_audit_t;
+/* k_marginal_path over the n distinct poses, then one CTA per factor (k_marginal_audit): Sigma_rel as
+ * asam_marginal_pairs forms it (bit-identical for the same J and poses), N = W - W Sigma_rel W (exactly symmetric),
+ * d2 = (W r)' N^-1 (W r) by a 3 x 3 Cholesky of N (NaN for a non-positive pivot) and redundancy = 3 - tr(Sigma_rel W).
+ * out: 11 doubles per factor, {d2, redundancy, Sigma_rel (row-major)}, host memory.  A factor's output depends only on
+ * its own record.  Writes only the scratch buffer; one H2D copy per table and one synchronisation. */
+int asam_marginal_audit(asam_dev_t *d, int n, const asam_marg_path_t *paths, int64_t z_doubles, int n_hops, int max_m,
+                        int k, const asam_marg_audit_t *recs, double *out);
+
 /* chi2 = sum 0.5 r'Wr (xyt, at state) + sum 0.5 rho(r'Wr) (robust xyt) + sum r'Wr (xytpos) over factors [0, n_factors)
  * using the st mirror (april_graph.c:79-98). Deterministic reduction. */
 int asam_chi2(asam_dev_t *d, int n_factors, double *chi2_out);
+/* Per factor of [first, first + count) at the st mirror: {r[3], s = r'Wr, w, chi2} (6 doubles, host memory), w the
+ * robust weight of a type-32 factor (1 otherwise) and chi2 the exact term asam_chi2 adds for the factor.  One D2H copy
+ * and one synchronisation. */
+int asam_factor_residuals(asam_dev_t *d, int first, int count, double *out);
 
 /* Status of the last factorisation: 0 ok, >0 = 1 + supernode id with a non-positive (or NaN) pivot,
  * <0 = internal dependency timeout.  A failed pivot turns its ancestors NaN, but they start only after their
@@ -250,6 +271,8 @@ int asam_debug_read_buffer(asam_dev_t *d, int id, int64_t off, int64_t bytes, vo
 void asam_debug_marginal_layout(int n, int64_t z_doubles, int n_hops, int64_t out5[5]);
 /* The same for an asam_marginal_pairs call: {out (10 doubles per candidate), paths, z, hops, pairs, total}. */
 void asam_debug_marginal_pairs_layout(int n, int64_t z_doubles, int n_hops, int k, int64_t out6[6]);
+/* The same for an asam_marginal_audit call: {out (11 doubles per factor), paths, z, hops, records, total}. */
+void asam_debug_marginal_audit_layout(int n, int64_t z_doubles, int n_hops, int k, int64_t out6[6]);
 int asam_sync(asam_dev_t *d);
 /* Counters: [0] kernel launches since creation, [1] bytes H2D, [2] bytes D2H. */
 int asam_counters(asam_dev_t *d, int64_t *out3);
