@@ -83,6 +83,14 @@ def lib() -> C.CDLL:
                                       C.c_void_p, _dp]
     L.asam_debug_marginal_audit_layout.argtypes = [C.c_int, C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_int64)]
     L.asam_debug_marginal_audit_layout.restype = None
+    L.aprilsam_b200_candidate_compatibility.argtypes = [C.c_void_p, C.c_void_p, C.c_int, _ip, _ip, _dp, _dp, _dp,
+                                                        _dp]
+    L.asam_marginal_compat.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
+                                       C.c_int, C.c_void_p, _ip, _dp, _dp]
+    L.asam_debug_marginal_compat_layout.argtypes = [C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int64,
+                                                    C.POINTER(C.c_int64)]
+    L.asam_debug_marginal_compat_layout.restype = None
+    L.asam_dbg_plan_compat_tiles.argtypes = [C.c_void_p, C.c_int, _ip, _ip, C.c_int64, _ip, C.c_int]
     L.aprilsam_b200_remove_factors.argtypes = [C.c_void_p, C.c_void_p, C.c_int, _ip, C.c_void_p]
     L.aprilsam_b200_relinearize_poses.argtypes = [C.c_void_p, C.c_void_p, C.c_int, _ip]
     L.asam_hessian_rebuild.argtypes = [C.c_void_p, C.c_int, _ip, _ip, C.c_int, _ip, _ip, C.c_int, _ip, _dp, _dp]

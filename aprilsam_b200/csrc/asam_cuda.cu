@@ -1537,6 +1537,30 @@ ASAM_EXPORT void asam_debug_marginal_audit_layout(int n, int64_t z_doubles, int 
         out6[q] = (int64_t) o[q];
 }
 
+// Byte offsets in the scratch of a compatibility tile: [err | out (10 doubles per record) | cross (10 doubles per pair
+// slot)] [paths] [z] [hops] [records] [ids]; err, out and cross come back with one copy.
+// o = {out, cross, paths, z, hops, records, ids, total}.
+static void marg_compat_layout(int n, int64_t z_doubles, int n_hops, int nc, int64_t slots, size_t o[8])
+{
+    o[0] = 16;
+    o[1] = o[0] + 10 * (size_t) nc * sizeof(double);
+    o[2] = align256(o[1] + 10 * (size_t) slots * sizeof(double));
+    o[3] = o[2] + align256((size_t) n * sizeof(asam_marg_path_t));
+    o[4] = o[3] + align256((size_t) z_doubles * sizeof(double));
+    o[5] = o[4] + align256(4 * (size_t) n_hops * sizeof(int));
+    o[6] = o[5] + align256((size_t) nc * sizeof(asam_marg_pair_t));
+    o[7] = o[6] + align256(2 * (size_t) nc * sizeof(int));
+}
+
+ASAM_EXPORT void asam_debug_marginal_compat_layout(int n, int64_t z_doubles, int n_hops, int nc, int64_t slots,
+                                                   int64_t out8[8])
+{
+    size_t o[8];
+    marg_compat_layout(n, z_doubles, n_hops, nc, slots, o);
+    for (int q = 0; q < 8; q++)
+        out8[q] = (int64_t) o[q];
+}
+
 // The dynamic shared memory limit of k_marginal_path is a property of the function on a device, shared by every
 // context (one per graph) in the process.  It only grows, so a launch sized at or below any value set before stays
 // valid while other threads query graphs with smaller fronts.
@@ -1713,6 +1737,69 @@ ASAM_EXPORT int asam_marginal_audit(asam_dev_t *d, int n, const asam_marg_path_t
         return set_err("asam_marginal_audit: %s", err == 1 ? "a front on a path is larger than max_m"
                                                             : "a path's length differs from the plan's");
     memcpy(out, host.data() + 2, 11 * (size_t) k * sizeof(double));
+    return 0;
+}
+
+ASAM_EXPORT int asam_marginal_compat(asam_dev_t *d, int n, const asam_marg_path_t *paths, int64_t z_doubles,
+                                     int n_hops, int max_m, int ni, int nj, int jo, const asam_marg_pair_t *recs,
+                                     const int *ids, double *out, double *cross)
+{
+    const int nc = jo + nj;
+    if (n < 1 || !paths || z_doubles < 3 || n_hops < n || max_m < 3 || ni < 1 || nj < 1 ||
+        (jo != 0 && jo != ni) || (jo == 0 && nj != ni) || (int64_t) ni * nj > INT32_MAX || !recs || !ids || !out ||
+        !cross)
+        return set_err("asam_marginal_compat: invalid arguments (n %d, z %lld, hops %d, max_m %d, ni %d, nj %d, jo %d)",
+                       n, (long long) z_doubles, n_hops, max_m, ni, nj, jo);
+    CK(cudaSetDevice(d->device));
+    const size_t smem = ASAM_MSMEM(max_m) * sizeof(double);
+    if (marg_smem_reserve(d->device, smem, max_m, "asam_marginal_compat"))
+        return 1;
+    const int64_t slots = (int64_t) ni * nj;
+    size_t lay[8];
+    marg_compat_layout(n, z_doubles, n_hops, nc, slots, lay);
+    const size_t out_bytes = lay[1] + 10 * (size_t) slots * sizeof(double);
+    if (buf_reserve(d, d->marg, lay[7], false, false))
+        return 1;
+    char *base = (char *) d->marg.p;
+    if (flush_uploads(d))
+        return 1;
+    CK(cudaMemcpyAsync(base + lay[2], paths, (size_t) n * sizeof(asam_marg_path_t), cudaMemcpyHostToDevice, d->stream));
+    CK(cudaMemcpyAsync(base + lay[5], recs, (size_t) nc * sizeof(asam_marg_pair_t), cudaMemcpyHostToDevice, d->stream));
+    CK(cudaMemcpyAsync(base + lay[6], ids, 2 * (size_t) nc * sizeof(int), cudaMemcpyHostToDevice, d->stream));
+    CK(cudaMemsetAsync(base, 0, 16, d->stream));
+    d->n_h2d += (int64_t) n * (int64_t) sizeof(asam_marg_path_t) + (int64_t) nc * (int64_t) sizeof(asam_marg_pair_t) +
+                2 * (int64_t) nc * (int64_t) sizeof(int);
+    MargArgs a;
+    a.sn = (const asam_sn_desc_t *) d->sn.p;
+    a.ipool = (const int *) d->ipool.p;
+    a.arena = (const double *) d->arena.p;
+    a.dinv = (const double *) d->dinv.p;
+    a.paths = (const asam_marg_path_t *) (base + lay[2]);
+    a.pairs = (const asam_marg_pair_t *) (base + lay[5]);
+    a.z = (double *) (base + lay[3]);
+    a.hop = (int *) (base + lay[4]);
+    a.out = (double *) (base + lay[0]);
+    a.err = (int *) base;
+    a.n = n;
+    a.max_m = max_m;
+    k_marginal_path<<<n, 256, smem, d->stream>>>(a);
+    CK(cudaGetLastError());
+    k_marginal_pairs<<<nc, 128, 0, d->stream>>>(a);
+    CK(cudaGetLastError());
+    k_marginal_compat<<<(unsigned) slots, 128, 0, d->stream>>>(a, (const int *) (base + lay[6]), ni, nj, jo,
+                                                                (double *) (base + lay[1]));
+    CK(cudaGetLastError());
+    d->n_launch += 3;
+    std::vector<double> host(out_bytes / sizeof(double));
+    if (download(d, host.data(), base, out_bytes))
+        return 1;
+    int err = 0;
+    memcpy(&err, host.data(), sizeof(int));
+    if (err)
+        return set_err("asam_marginal_compat: %s", err == 1 ? "a front on a path is larger than max_m"
+                                                             : "a path's length differs from the plan's");
+    memcpy(out, host.data() + 2, 10 * (size_t) nc * sizeof(double));
+    memcpy(cross, host.data() + lay[1] / sizeof(double), 10 * (size_t) slots * sizeof(double));
     return 0;
 }
 

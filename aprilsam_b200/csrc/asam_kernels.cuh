@@ -3227,3 +3227,134 @@ __global__ void __launch_bounds__(128) k_marginal_audit(MargArgs a, const asam_m
     for (int q = 0; q < 9; q++)
         o[2 + q] = R[q];
 }
+
+// Whether tile record q precedes record p in a pair's canonical order: (a, b) node ids (ids, 2 per record), then the
+// bits of r and of Winv.  Two records that compare equal hold the same inputs, so either order gives the same bits:
+// the pair's output depends only on the two candidates, not on where the request put them.
+__device__ __forceinline__ bool compat_precedes(const asam_marg_pair_t *rec, const int *ids, int q, int p)
+{
+    for (int e = 0; e < 2; e++)
+        if (ids[2 * q + e] != ids[2 * p + e])
+            return ids[2 * q + e] < ids[2 * p + e];
+    for (int e = 0; e < 3; e++) {
+        const long long u = __double_as_longlong(rec[q].r[e]), v = __double_as_longlong(rec[p].r[e]);
+        if (u != v)
+            return u < v;
+    }
+    for (int e = 0; e < 9; e++) {
+        const long long u = __double_as_longlong(rec[q].Winv[e]), v = __double_as_longlong(rec[p].Winv[e]);
+        if (u != v)
+            return u < v;
+    }
+    return false;
+}
+
+// One CTA per pair slot (li, lj) of a compatibility tile, after k_marginal_path and k_marginal_pairs on the tile's
+// records (a.pairs; a.out holds k_marginal_pairs' 10 doubles per record).  Records [0, ni) are the tile's rows I,
+// [jo, jo + nj) its columns J; jo = 0 is a diagonal tile (J = I), where only li < lj is a pair.  With f, s the pair
+// in canonical order (compat_precedes), on one thread:
+//   Sigma(poses of f, poses of s) by marg_block: 4 blocks for two closures, 2 with one prior, 1 for two priors;
+//   C = J_f Sigma J_s' (a row-major 3 x 6 by 6 x 6 by 6 x 3 product; J = [I 0] of a prior takes the rows / columns of
+//   its pose directly);
+//   S = [S_f C; C' S_s], S_c = Sigma_rel,c + Winv_c from k_marginal_pairs' Sigma_rel as it forms S;
+//   S = L L' column by column, d2 = |L^-1 [r_f; r_s]|^2 (NaN for a pivot that is not > 0).
+// cross: 10 doubles per slot li * nj + lj, {d2, C_ij (row-major, i the row candidate)}.  No floating-point atomics;
+// a pair's output depends only on its two records.
+__global__ void __launch_bounds__(128) k_marginal_compat(MargArgs a, const int *ids, int ni, int nj, int jo,
+                                                         double *cross)
+{
+    const int tid = threadIdx.x;
+    const int p = blockIdx.x, li = p / nj, lj = p % nj;
+    if (jo == 0 && li >= lj)
+        return;
+    const int ci = li, cj = jo + lj;
+    const bool sw = compat_precedes(a.pairs, ids, cj, ci);
+    const int f = sw ? cj : ci, s = sw ? ci : cj;
+    const asam_marg_pair_t &F = a.pairs[f], &G = a.pairs[s];
+    const int nf = F.pb >= 0 ? 2 : 1, ns = G.pb >= 0 ? 2 : 1;
+    __shared__ double sg[2][2][9]; // Sigma(pose u of f, pose v of s), u, v: 0 = a, 1 = b
+    for (int u = 0; u < nf; u++)
+        for (int v = 0; v < ns; v++) {
+            const int pu = u ? F.pb : F.pa, pv = v ? G.pb : G.pa;
+            const double x = marg_block(a, a.paths[pu], a.paths[pv], pu == pv);
+            if (tid < 9)
+                sg[u][v][tid] = x;
+        }
+    __syncthreads();
+    if (tid != 0)
+        return;
+    // Sigma (3 nf x 3 ns), entry (r, c)
+    auto X = [&](int r, int c) -> double { return sg[r / 3][c / 3][3 * (r % 3) + c % 3]; };
+    double T[18]; // J_f Sigma, 3 x 3 ns
+    for (int r = 0; r < 3; r++)
+        for (int c = 0; c < 3 * ns; c++) {
+            if (nf == 1) {
+                T[6 * r + c] = X(r, c);
+            } else {
+                double acc = 0.0;
+                for (int k = 0; k < 6; k++)
+                    acc += F.J[6 * r + k] * X(k, c);
+                T[6 * r + c] = acc;
+            }
+        }
+    double C[9]; // C_fs = J_f Sigma J_s'
+    for (int r = 0; r < 3; r++)
+        for (int c = 0; c < 3; c++) {
+            if (ns == 1) {
+                C[3 * r + c] = T[6 * r + c];
+            } else {
+                double acc = 0.0;
+                for (int k = 0; k < 6; k++)
+                    acc += T[6 * r + k] * G.J[6 * c + k];
+                C[3 * r + c] = acc;
+            }
+        }
+    // the lower triangle of S, row-major in M[6][6]
+    double M[6][6];
+    const double *Rf = a.out + 10 * (size_t) f + 1, *Rs = a.out + 10 * (size_t) s + 1;
+#pragma unroll
+    for (int r = 0; r < 3; r++)
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            M[r][c] = Rf[3 * r + c] + F.Winv[3 * r + c];
+            M[3 + r][3 + c] = Rs[3 * r + c] + G.Winv[3 * r + c];
+            M[3 + r][c] = C[3 * c + r];
+        }
+    double L[6][6], y[6];
+    const double rhs[6] = {F.r[0], F.r[1], F.r[2], G.r[0], G.r[1], G.r[2]};
+#pragma unroll
+    for (int j = 0; j < 6; j++) {
+        double e = M[j][j];
+#pragma unroll
+        for (int k = 0; k < j; k++)
+            e -= L[j][k] * L[j][k];
+        L[j][j] = e > 0.0 ? sqrt(e) : nan("");
+#pragma unroll
+        for (int i = j + 1; i < 6; i++) {
+            double v = M[i][j];
+#pragma unroll
+            for (int k = 0; k < j; k++)
+                v -= L[i][k] * L[j][k];
+            L[i][j] = v / L[j][j];
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < 6; i++) {
+        double v = rhs[i];
+#pragma unroll
+        for (int k = 0; k < i; k++)
+            v -= L[i][k] * y[k];
+        y[i] = v / L[i][i];
+    }
+    double d2 = y[0] * y[0];
+#pragma unroll
+    for (int i = 1; i < 6; i++)
+        d2 += y[i] * y[i];
+    double *o = cross + 10 * (size_t) p;
+    o[0] = d2;
+#pragma unroll
+    for (int r = 0; r < 3; r++)
+#pragma unroll
+        for (int c = 0; c < 3; c++)
+            o[1 + 3 * r + c] = sw ? C[3 * c + r] : C[3 * r + c];
+}

@@ -75,6 +75,7 @@ def _load(impl: str) -> C.CDLL:
     for name, args in (("h_marginal_cov", [C.c_void_p, C.c_int, _ip, _dp]),
                        ("h_relative_cov", [C.c_void_p, C.c_int, C.c_int, _dp]),
                        ("h_candidate_mahalanobis", [C.c_void_p, C.c_int, _ip, _ip, _dp, _dp, _dp, _dp]),
+                       ("h_candidate_compatibility", [C.c_void_p, C.c_int, _ip, _ip, _dp, _dp, _dp, _dp]),
                        ("h_factor_residuals", [C.c_void_p, C.c_int, C.c_int, _dp]),
                        ("h_factor_outlier_scores", [C.c_void_p, C.c_int, _ip, _dp, _dp, _dp]),
                        ("h_remove_factors", [C.c_void_p, C.c_int, _ip, C.c_int]),
@@ -278,6 +279,26 @@ class Harness:
                                             _d(cov) if with_cov else None) != 0:
             raise RuntimeError(self.lib.aprilsam_b200_last_error().decode())
         return (d2, cov) if with_cov else d2
+
+    def candidate_compatibility(self, a, b, z, W, with_cross: bool = False):
+        """aprilsam_b200_candidate_compatibility: d2 (k, k) of the candidates' pairs (diagonal: each candidate's own
+        candidate_mahalanobis d2; off the diagonal: the joint distance of the pair, 6 degrees of freedom); with_cross
+        also returns C (k, k, 3, 3), the cross-covariances of the residuals (C[c, c] = Sigma_rel of c).  Candidates as
+        for candidate_mahalanobis.  Raises RuntimeError with the library's message when it returns -1."""
+        a = np.ascontiguousarray(a, dtype=np.int32).reshape(-1)
+        b = np.ascontiguousarray(b, dtype=np.int32).reshape(-1)
+        k = len(a)
+        if len(b) != k:
+            raise ValueError(f"a has {k} ids, b {len(b)}")
+        z = np.ascontiguousarray(z, dtype=np.float64).reshape(k, 3)
+        W = np.ascontiguousarray(W, dtype=np.float64).reshape(k, 9)
+        n = max(k, 1)
+        d2 = np.zeros((n, n), dtype=np.float64)
+        cross = np.zeros((n, n, 3, 3), dtype=np.float64) if with_cross else None
+        if self.lib.h_candidate_compatibility(self.h, k, _i(a), _i(b), _d(z), _d(W), _d(d2),
+                                              _d(cross) if with_cross else None) != 0:
+            raise RuntimeError(self.lib.aprilsam_b200_last_error().decode())
+        return (d2[:k, :k], cross[:k, :k]) if with_cross else d2[:k, :k]
 
     def factor_residuals(self, first: int = 0, count=None):
         """aprilsam_b200_factor_residuals: (count, 6) rows {r[0], r[1], r[2], s = r'Wr, w, chi2} of factors

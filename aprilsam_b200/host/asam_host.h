@@ -198,6 +198,17 @@ int plan_marginal_paths(const plan_t *pl, int n, const int *nodes, asam_marg_pat
 void plan_candidate_batches(const plan_t *pl, int k, const int *a, const int *b, int64_t budget, int *batch_end,
                             int *n_batches, int *poses, int *pose_end, int *ia, int *ib);
 
+/* Tiles of a candidate compatibility query (aprilsam_b200_candidate_compatibility) over candidates (a[c], b[c]) as
+ * for plan_candidate_batches: tile t is {i0, i1, j0, j1} (4 ints of *tiles_out, malloc'ed, the caller frees it), the
+ * pairs (i, j) of [i0, i1) x [j0, j1) with i <= j.  A diagonal tile has i0 = j0 and i1 = j1; otherwise i1 <= j0.
+ * Every pair i <= j lies in exactly one tile, and so does every diagonal pair (c, c).  The scratch of a tile, the z
+ * rows of the distinct poses of its candidates plus 10 doubles per slot (i1 - i0) x (j1 - j0), stays within `budget`
+ * doubles unless the tile holds a single pair.  When the whole request fits, there is one tile [0, k) x [0, k).
+ * Otherwise the candidates split, in input order, into blocks whose own poses take at most a quarter of the budget
+ * and whose slots at most half, and tile (B_p, B_q) is a pair of blocks, p <= q.  Returns the number of tiles.  A
+ * pure function of the plan, the ids and the budget. */
+int plan_compat_tiles(const plan_t *pl, int k, const int *a, const int *b, int64_t budget, int **tiles_out);
+
 /* Bytes of z scratch a batch of a candidate query may take (solver.c; tests lower it through debug.c) */
 #define ASAM_CANDIDATE_BUDGET ((int64_t) 256 << 20)
 extern int64_t asam_candidate_budget;

@@ -38,6 +38,18 @@ ASAM_API int asam_dbg_plan_candidate_batches(void *p, int k, const int *a, const
     return nb;
 }
 
+/* plan_compat_tiles on a plan: returns the number of tiles and writes up to cap of them (4 ints each) */
+ASAM_API int asam_dbg_plan_compat_tiles(void *p, int k, const int *a, const int *b, int64_t budget_doubles, int *tiles,
+                                        int cap)
+{
+    int *t = NULL;
+    const int nt = plan_compat_tiles((const plan_t *) p, k, a, b, budget_doubles, &t);
+    if (tiles && cap > 0)
+        memcpy(tiles, t, sizeof(int) * 4 * (size_t) (nt < cap ? nt : cap));
+    free(t);
+    return nt;
+}
+
 /* the residual helpers of graph.c: an xyt factor at (pa, pb), an xytpos factor at pa (pb NULL) */
 ASAM_API void asam_dbg_residual(const double *z, const double *pa, const double *pb, double *r)
 {

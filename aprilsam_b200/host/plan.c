@@ -2056,3 +2056,104 @@ void plan_candidate_batches(const plan_t *pl, int k, const int *a, const int *b,
     free(slot);
     *n_batches = nb;
 }
+
+/* scratch doubles of the distinct poses of candidates [c0, c1) and [d0, d1); slot (all -1) is left as it was found */
+static int64_t compat_union_doubles(const plan_t *pl, int *slot, const int *a, const int *b, int c0, int c1, int d0,
+                                    int d1)
+{
+    int64_t z = 0;
+    for (int pass = 0; pass < 2; pass++)
+        for (int h = 0; h < 2; h++)
+            for (int c = h ? d0 : c0; c < (h ? d1 : c1); c++)
+                for (int e = 0; e < 2; e++) {
+                    const int node = e ? b[c] : a[c];
+                    if (node < 0)
+                        continue;
+                    if (pass == 1) {
+                        slot[node] = -1;
+                    } else if (slot[node] < 0) {
+                        slot[node] = 0;
+                        z += marginal_path_doubles(pl, pl->node2q[node]);
+                    }
+                }
+    return z;
+}
+
+/* the scratch of tile (I, J): the z rows of its distinct poses and 10 doubles per pair slot |I| x |J| */
+static int64_t compat_tile_doubles(const plan_t *pl, int *slot, const int *a, const int *b, int i0, int i1, int j0,
+                                   int j1)
+{
+    return compat_union_doubles(pl, slot, a, b, i0, i1, j0, j1) + 10 * (int64_t) (i1 - i0) * (int64_t) (j1 - j0);
+}
+
+static void compat_push(int **t, int *n, int *cap, int i0, int i1, int j0, int j1)
+{
+    if (*n == *cap) {
+        *cap = *cap ? 2 * *cap : 16;
+        *t = realloc(*t, sizeof(int) * 4 * (size_t) *cap);
+    }
+    int *q = *t + 4 * (size_t) (*n)++;
+    q[0] = i0;
+    q[1] = i1;
+    q[2] = j0;
+    q[3] = j1;
+}
+
+int plan_compat_tiles(const plan_t *pl, int k, const int *a, const int *b, int64_t budget, int **tiles_out)
+{
+    int *slot = malloc(sizeof(int) * (size_t) (pl->N > 0 ? pl->N : 1));
+    for (int i = 0; i < pl->N; i++)
+        slot[i] = -1;
+    int *t = NULL, nt = 0, cap = 0;
+    if (compat_tile_doubles(pl, slot, a, b, 0, k, 0, k) <= budget) {
+        compat_push(&t, &nt, &cap, 0, k, 0, k);
+    } else {
+        /* blocks in input order: each within a quarter of the budget in z and half of it in pair slots, so that any
+         * two of them make a tile within the budget */
+        int *bend = malloc(sizeof(int) * (size_t) k), nb = 0, c0 = 0, p0 = 0, np = 0;
+        int *bp = malloc(sizeof(int) * 2 * (size_t) k);
+        int64_t z = 0;
+        for (int c = 0; c < k; c++) {
+            int64_t ext = candidate_new_doubles(pl, slot, a[c], b[c]);
+            const int64_t n1 = c - c0 + 1;
+            if (c > c0 && (z + ext > budget / 4 || 10 * n1 * n1 > budget / 2)) {
+                for (int i = p0; i < np; i++)
+                    slot[bp[i]] = -1;
+                bend[nb++] = c;
+                c0 = c;
+                p0 = np;
+                z = 0;
+                ext = candidate_new_doubles(pl, slot, a[c], b[c]);
+            }
+            z += ext;
+            for (int e = 0; e < 2; e++) {
+                const int node = e ? b[c] : a[c];
+                if (node >= 0 && slot[node] < 0) {
+                    slot[node] = 0;
+                    bp[np++] = node;
+                }
+            }
+        }
+        for (int i = p0; i < np; i++)
+            slot[bp[i]] = -1;
+        bend[nb++] = k;
+        /* tiles (B_p, B_q), p <= q; a pair of blocks beyond the budget (one of them a single candidate that alone
+         * exceeds its share) goes one pair per tile */
+        for (int p = 0; p < nb; p++)
+            for (int q = p; q < nb; q++) {
+                const int i0 = p ? bend[p - 1] : 0, i1 = bend[p], j0 = q ? bend[q - 1] : 0, j1 = bend[q];
+                if (p == q || compat_tile_doubles(pl, slot, a, b, i0, i1, j0, j1) <= budget) {
+                    compat_push(&t, &nt, &cap, i0, i1, j0, j1);
+                    continue;
+                }
+                for (int i = i0; i < i1; i++)
+                    for (int j = j0; j < j1; j++)
+                        compat_push(&t, &nt, &cap, i, i + 1, j, j + 1);
+            }
+        free(bend);
+        free(bp);
+    }
+    free(slot);
+    *tiles_out = t;
+    return nt;
+}

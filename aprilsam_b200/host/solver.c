@@ -2324,20 +2324,12 @@ static int candidates_run(solver_t *s, int k, const int *a, const int *b, asam_m
     return rc;
 }
 
-ASAM_API int aprilsam_b200_candidate_mahalanobis(april_graph_t *g, april_graph_cholesky_param_t *param, int k,
-                                                 const int *a, const int *b, const double *z, const double *W,
-                                                 double *d2, double *cov9)
+/* The records of k candidates (J, r, Winv, has_w; pa / pb are set per batch): 0, or -1 with the error text for the
+ * first candidate at fault */
+static int candidate_records(solver_t *s, april_graph_t *g, int k, const int *a, const int *b, const double *z,
+                             const double *W, asam_marg_pair_t *rec, const char *fn)
 {
-    const char *fn = "aprilsam_b200_candidate_mahalanobis";
-    if (k < 1 || !a || !b || !z || !W || !d2) {
-        asam_set_error("%s: NULL a / b / z / W / d2 or k < 1", fn);
-        return -1;
-    }
-    solver_t *s = marginal_solver(g, param, fn);
-    if (!s)
-        return -1;
     const int N = s->plan.N;
-    asam_marg_pair_t *rec = calloc((size_t) k, sizeof(*rec));
     int rc = 0;
     for (int c = 0; c < k && rc == 0; c++) {
         const double *zc = z + 3 * (size_t) c;
@@ -2366,6 +2358,23 @@ ASAM_API int aprilsam_b200_candidate_mahalanobis(april_graph_t *g, april_graph_c
             asam_xytpos_residual(zc, sa, rec[c].r);
         }
     }
+    return rc;
+}
+
+ASAM_API int aprilsam_b200_candidate_mahalanobis(april_graph_t *g, april_graph_cholesky_param_t *param, int k,
+                                                 const int *a, const int *b, const double *z, const double *W,
+                                                 double *d2, double *cov9)
+{
+    const char *fn = "aprilsam_b200_candidate_mahalanobis";
+    if (k < 1 || !a || !b || !z || !W || !d2) {
+        asam_set_error("%s: NULL a / b / z / W / d2 or k < 1", fn);
+        return -1;
+    }
+    solver_t *s = marginal_solver(g, param, fn);
+    if (!s)
+        return -1;
+    asam_marg_pair_t *rec = calloc((size_t) k, sizeof(*rec));
+    int rc = candidate_records(s, g, k, a, b, z, W, rec, fn);
     if (rc == 0)
         rc = candidates_run(s, k, a, b, rec, d2, cov9, fn);
     free(rec);
@@ -2396,6 +2405,113 @@ ASAM_API int aprilsam_b200_relative_covariance(april_graph_t *g, april_graph_cho
     candidate_jacobian(g, a, b, rec.J);
     double d2;
     return candidates_run(s, 1, &a, &b, &rec, &d2, out9, fn);
+}
+
+/* ---- candidate compatibility: joint Mahalanobis distances of candidate pairs (extension) ---------------------- */
+/* One tile of plan_compat_tiles: the distinct poses of its candidates, the tile's records with pa / pb into them, one
+ * asam_marginal_compat, and its outputs scattered into d2 / cross9 (k x k) */
+static int compat_tile(solver_t *s, int k, const int *a, const int *b, const asam_marg_pair_t *rec,
+                       const int *tile, int *slot, double *d2, double *cross9, const char *fn)
+{
+    const plan_t *pl = &s->plan;
+    const int i0 = tile[0], ni = tile[1] - tile[0], j0 = tile[2], nj = tile[3] - tile[2];
+    const int jo = i0 == j0 ? 0 : ni, nc = jo + nj;
+    int *poses = malloc(sizeof(int) * 2 * (size_t) nc), *ids = malloc(sizeof(int) * 2 * (size_t) nc);
+    asam_marg_pair_t *tr = malloc(sizeof(*tr) * (size_t) nc);
+    asam_marg_path_t *paths = malloc(sizeof(*paths) * 2 * (size_t) nc);
+    double *out = malloc(sizeof(double) * 10 * (size_t) nc);
+    double *cross = malloc(sizeof(double) * 10 * (size_t) ni * (size_t) nj);
+    int np = 0, rc = 0;
+    for (int l = 0; l < nc; l++) {
+        const int c = l < ni ? i0 + l : j0 + (l - jo);
+        tr[l] = rec[c];
+        ids[2 * l] = a[c];
+        ids[2 * l + 1] = b[c];
+        for (int e = 0; e < 2; e++) {
+            const int node = e ? b[c] : a[c];
+            if (node >= 0 && slot[node] < 0) {
+                slot[node] = np;
+                poses[np++] = node;
+            }
+        }
+        tr[l].pa = slot[a[c]];
+        tr[l].pb = b[c] >= 0 ? slot[b[c]] : -1;
+    }
+    for (int i = 0; i < np; i++)
+        slot[poses[i]] = -1;
+    int64_t z = 0;
+    int hops = 0;
+    if (plan_marginal_paths(pl, np, poses, paths, &z, &hops) != 0) {
+        char why[512];
+        snprintf(why, sizeof(why), "%s", g_error);
+        asam_set_error("%s: %s", fn, why);
+        rc = -1;
+    } else if (asam_marginal_compat(s->gc->dev, np, paths, z, hops, pl->max_m, ni, nj, jo, tr, ids, out, cross) != 0) {
+        asam_set_error("%s: %s", fn, asam_last_error());
+        rc = -1;
+    }
+    for (int li = 0; li < ni && rc == 0; li++) {
+        const int i = i0 + li;
+        if (jo == 0) { /* the diagonal: the candidate query's own d2 and Sigma_rel */
+            d2[(size_t) i * k + i] = out[10 * (size_t) li];
+            if (cross9)
+                memcpy(cross9 + 9 * ((size_t) i * k + i), out + 10 * (size_t) li + 1, 9 * sizeof(double));
+        }
+        for (int lj = jo ? 0 : li + 1; lj < nj; lj++) {
+            const int j = j0 + lj;
+            const double *o = cross + 10 * ((size_t) li * nj + lj);
+            d2[(size_t) i * k + j] = d2[(size_t) j * k + i] = o[0];
+            if (cross9) {
+                double *cij = cross9 + 9 * ((size_t) i * k + j), *cji = cross9 + 9 * ((size_t) j * k + i);
+                for (int r = 0; r < 3; r++)
+                    for (int q = 0; q < 3; q++) {
+                        cij[3 * r + q] = o[1 + 3 * r + q];
+                        cji[3 * q + r] = o[1 + 3 * r + q];
+                    }
+            }
+        }
+    }
+    free(poses);
+    free(ids);
+    free(tr);
+    free(paths);
+    free(out);
+    free(cross);
+    return rc;
+}
+
+ASAM_API int aprilsam_b200_candidate_compatibility(april_graph_t *g, april_graph_cholesky_param_t *param, int k,
+                                                   const int *a, const int *b, const double *z, const double *W,
+                                                   double *d2, double *cross9)
+{
+    const char *fn = "aprilsam_b200_candidate_compatibility";
+    if (k < 1 || !a || !b || !z || !W || !d2) {
+        asam_set_error("%s: NULL a / b / z / W / d2 or k < 1", fn);
+        return -1;
+    }
+    if (k > APRILSAM_B200_COMPAT_MAX_K) {
+        asam_set_error("%s: k = %d candidates; at most %d (k * k pair slots are indexed by int)", fn, k,
+                       APRILSAM_B200_COMPAT_MAX_K);
+        return -1;
+    }
+    solver_t *s = marginal_solver(g, param, fn);
+    if (!s)
+        return -1;
+    asam_marg_pair_t *rec = calloc((size_t) k, sizeof(*rec));
+    int rc = candidate_records(s, g, k, a, b, z, W, rec, fn);
+    if (rc == 0) {
+        int *tiles = NULL;
+        const int nt = plan_compat_tiles(&s->plan, k, a, b, asam_candidate_budget / (int64_t) sizeof(double), &tiles);
+        int *slot = malloc(sizeof(int) * (size_t) s->plan.N);
+        for (int i = 0; i < s->plan.N; i++)
+            slot[i] = -1;
+        for (int t = 0; t < nt && rc == 0; t++)
+            rc = compat_tile(s, k, a, b, rec, tiles + 4 * (size_t) t, slot, d2, cross9, fn);
+        free(slot);
+        free(tiles);
+    }
+    free(rec);
+    return rc;
 }
 
 /* ---- factor audit: leave-one-out Mahalanobis distances and redundancies (extension) ---------------------------- */

@@ -576,6 +576,13 @@ H_EXPORT int h_candidate_mahalanobis(hctx_t *h, int k, const int *a, const int *
     return aprilsam_b200_candidate_mahalanobis(h->g, h->p, k, a, b, z, W, d2, cov9);
 }
 
+/* aprilsam_b200_candidate_compatibility (d2: k x k; cross9: k x k x 9 or NULL) */
+H_EXPORT int h_candidate_compatibility(hctx_t *h, int k, const int *a, const int *b, const double *z, const double *W,
+                                       double *d2, double *cross9)
+{
+    return aprilsam_b200_candidate_compatibility(h->g, h->p, k, a, b, z, W, d2, cross9);
+}
+
 /* aprilsam_b200_factor_residuals (out: 6 doubles per factor) / _factor_outlier_scores */
 H_EXPORT int h_factor_residuals(hctx_t *h, int first, int count, double *out)
 {

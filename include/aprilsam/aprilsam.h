@@ -313,6 +313,46 @@ int aprilsam_b200_relative_covariance(april_graph_t *graph, april_graph_cholesky
 int aprilsam_b200_candidate_mahalanobis(april_graph_t *graph, april_graph_cholesky_param_t *param, int k, const int *a,
                                         const int *b, const double *z, const double *W, double *d2, double *cov9);
 
+/* ---- candidate compatibility (extension) ---------------------------------------------------------------------------
+ * Which candidates can be true together.  aprilsam_b200_candidate_mahalanobis tests each candidate on its own; on a
+ * long loop Sigma_rel is large, so a false closure from perceptual aliasing (a corridor, a row of doors, a repeated
+ * room) passes that gate, and usually several pass together.  Their residuals share one drift, because the Sigma_rel of
+ * neighbouring closures are strongly correlated: two closures that each sit inside their own ellipse can pull that
+ * drift in opposite directions.  Testing them jointly catches this (pairwise compatibility and a maximum clique, as in
+ * CCDA or PCM; or joint compatibility, JCBB).
+ *
+ * aprilsam_b200_candidate_compatibility: for k candidates exactly as aprilsam_b200_candidate_mahalanobis takes them
+ * (a[c], b[c], z, W; b[c] = -1 for a prior on a[c]; r at the states, J at the l_points; the same validation and error
+ * texts), with Sigma as aprilsam_b200_marginal_covariance defines it and J = [I 0] for a prior:
+ *   C_ij = J_i Sigma_(a_i b_i),(a_j b_j) J_j'      the cross-covariance of the two residuals
+ *   S_i  = Sigma_rel,i + W_i^-1
+ *   d2[i*k + j] = [r_i; r_j]' S_ij^-1 [r_i; r_j],  S_ij = [S_i C_ij; C_ij' S_j]   (i != j)
+ *   d2[c*k + c] = the d2 aprilsam_b200_candidate_mahalanobis returns for c, bit for bit.
+ * d2 is k x k, row-major and exactly symmetric.  Compare an off-diagonal entry with a chi-square quantile with 6
+ * degrees of freedom: 16.81 (99 %), 22.46 (99.9 %).  It is NaN when S_ij is not numerically positive definite (a
+ * pivot of its 6 x 6 Cholesky is not > 0).  In the linear model d2[i*k + j] = d2_i + d2_(j|i), d2_(j|i) the candidate
+ * distance of j against the solve with i added, and d2[i*k + j] >= max(d2_i, d2_j).
+ *
+ * cross9 (NULL allowed): C_ij for every ordered pair, k x k x 9 doubles, each block row-major; cross9 at (j, i) is the
+ * exact transpose of (i, j), and cross9 at (c, c) is Sigma_rel of c, the cov9 of aprilsam_b200_candidate_mahalanobis,
+ * bit for bit.  With it a caller can run JCBB on any subset: S of a set is these blocks plus W^-1 on the diagonal.
+ *
+ * An entry (i, j) depends only on candidates i and j: the same bits for the pair alone (k = 2), inside any request, in
+ * any order (a permutation of the input permutes the matrix), under any tiling and from call to call.  The pairs are
+ * computed in tiles whose query scratch stays within the candidate query's budget (256 MiB); each tile walks the root
+ * paths of its distinct poses once, and when the whole request fits, every distinct pose is walked once.  The cost
+ * grows with k^2 (one small 6 x 6 problem and up to four 3 x 3 blocks of Sigma per pair) plus the path walks; nothing
+ * but the query scratch on the GPU is written.
+ *
+ * Returns 0, or -1 with the reason in aprilsam_b200_last_error() and nothing changed for everything
+ * aprilsam_b200_candidate_mahalanobis refuses and for k > APRILSAM_B200_COMPAT_MAX_K (checked before d2 is touched):
+ * the kernel indexes a tile's k x k pair slots with an int.  d2 and cross9 are unspecified after an error; the solver
+ * stays usable. */
+#define APRILSAM_B200_COMPAT_MAX_K 46340
+int aprilsam_b200_candidate_compatibility(april_graph_t *graph, april_graph_cholesky_param_t *param, int k,
+                                          const int *a, const int *b, const double *z, const double *W, double *d2,
+                                          double *cross9);
+
 /* ---- factor audit (extension) ------------------------------------------------------------------------------------
  * Which accepted factor has proved false.  A raw residual is the wrong test: the solve pulls the graph towards an
  * outlier, so its residual shrinks, and a factor the rest of the graph hardly checks looks good even when it is wrong.

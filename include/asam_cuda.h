@@ -236,6 +236,20 @@ typedef struct asam_marg_audit {
  * its own record.  Writes only the scratch buffer; one H2D copy per table and one synchronisation. */
 int asam_marginal_audit(asam_dev_t *d, int n, const asam_marg_path_t *paths, int64_t z_doubles, int n_hops, int max_m,
                         int k, const asam_marg_audit_t *recs, double *out);
+/* One tile of a candidate compatibility query: k_marginal_path over the n distinct poses of the tile, k_marginal_pairs
+ * over its nc = jo + nj records (recs[c].pa / pb index paths; has_w = 1), then one CTA per pair slot
+ * (k_marginal_compat).  Records [0, ni) are the rows I, [jo, jo + nj) the columns J: jo = 0 is a diagonal tile
+ * (nj = ni, J = I, pairs li < lj), jo = ni an off-diagonal one (every slot a pair); ni * nj <= INT32_MAX (one CTA per
+ * slot).  ids: the a and b node ids of each record (2 ints), the key of a pair's canonical order.  For a pair (i, j):
+ * the cross blocks of Sigma between the candidates' poses by marg_block, C_ij = J_i Sigma J_j' (J = [I 0] of a prior),
+ * S = [S_i C_ij; C_ij' S_j] with S_c = Sigma_rel,c + Winv_c as k_marginal_pairs forms it, a 6 x 6 Cholesky of S and
+ * d2 = |L^-1 [r_i; r_j]|^2 (NaN for a pivot that is not > 0).  out (host memory): k_marginal_pairs' 10 doubles per
+ * record ({d2, Sigma_rel}, as asam_marginal_pairs returns them); cross (host memory): 10 doubles per slot
+ * li * nj + lj, {d2, C_ij row-major} (unwritten for li >= lj of a diagonal tile).  A pair's output depends only on its
+ * two records.  Writes only the scratch buffer; one H2D copy per table and one synchronisation. */
+int asam_marginal_compat(asam_dev_t *d, int n, const asam_marg_path_t *paths, int64_t z_doubles, int n_hops, int max_m,
+                         int ni, int nj, int jo, const asam_marg_pair_t *recs, const int *ids, double *out,
+                         double *cross);
 
 /* chi2 = sum 0.5 r'Wr (xyt, at state) + sum 0.5 rho(r'Wr) (robust xyt) + sum r'Wr (xytpos) over factors [0, n_factors)
  * using the st mirror (april_graph.c:79-98). Deterministic reduction. */
@@ -273,6 +287,9 @@ void asam_debug_marginal_layout(int n, int64_t z_doubles, int n_hops, int64_t ou
 void asam_debug_marginal_pairs_layout(int n, int64_t z_doubles, int n_hops, int k, int64_t out6[6]);
 /* The same for an asam_marginal_audit call: {out (11 doubles per factor), paths, z, hops, records, total}. */
 void asam_debug_marginal_audit_layout(int n, int64_t z_doubles, int n_hops, int k, int64_t out6[6]);
+/* The same for an asam_marginal_compat tile of nc records and `slots` pair slots: {out (10 doubles per record), cross
+ * (10 doubles per slot), paths, z, hops, records, ids, total}. */
+void asam_debug_marginal_compat_layout(int n, int64_t z_doubles, int n_hops, int nc, int64_t slots, int64_t out8[8]);
 int asam_sync(asam_dev_t *d);
 /* Counters: [0] kernel launches since creation, [1] bytes H2D, [2] bytes D2H. */
 int asam_counters(asam_dev_t *d, int64_t *out3);
